@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark: greedy generate through ``DistributedModel`` on N B200s (pipeline-sharded), tokens/s.
+"""Headline benchmark: greedy generate through ``DistributedModel`` on N H100s (pipeline-sharded), tokens/s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload qwen2.5-7b|qwen2.5-0.5b|...] [--impl reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -10,6 +10,12 @@ batch (global batch = rows_per_gpu x N micro-batches rotating through the N pipe
 ``value`` = generated tokens / device time with the prompt already in HBM; ``e2e`` = the same through the public
 API from pinned host memory to host memory.  ``--impl reference`` times the reference's CPU shard math (the oracle
 port, all host threads) on a bounded sample of the same workload.
+
+``--dump-outputs DIR`` writes, after the timed steps, what the last timed step returned to its caller: the generated
+token ids (``DIR/tokens.npy``) and, unless ``--no-train``, the last training step's loss (``DIR/train_loss.npy``) and a
+fixed, seeded sample of 4096 elements of every parameter and every gradient that step left behind
+(``DIR/train_params_sample.npy``, ``DIR/train_grads_sample.npy``), all float64.  Weights and inputs are seeded, so two builds run with the same arguments can be compared output for
+output.
 """
 import argparse
 import json
@@ -41,7 +47,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "measured"
-    return 6650.0, 1590.0, "fallback"
+    return 3350.0, 989.0, "H100 SXM data-sheet"
 
 
 def burst_tflops(default):
@@ -53,7 +59,7 @@ def burst_tflops(default):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -317,7 +323,7 @@ def measure_gemv_launches(dm, rows):
                          ("o", lambda: nat.gemv(w.attn, v[f"l{li}.wo"], out=x, residual=x)),
                          ("gate_up", lambda: nat.gemv(x, v[f"l{li}.wgu"], out=w.act, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, flags=nat.EPI_SWIGLU)),
                          ("down", lambda: nat.gemv(w.act, v[f"l{li}.wd"], out=x, residual=x)))
-            else:       # batched decode streams the weights through the tcgen05 GEMM (M = rows)
+            else:       # batched decode streams the weights through the wgmma GEMM (M = rows)
                 calls = (("qkv", lambda: nat.gemm(x, v[f"l{li}.wqkv"], out=w.qkv, bias=v.get(f"l{li}.bqkv"))),
                          ("o", lambda: nat.gemm(w.attn, v[f"l{li}.wo"], out=x, residual=x)),
                          ("gate_up", lambda: nat.gemm(x, v[f"l{li}.wgu"], out=w.act, flags=nat.EPI_SWIGLU)),
@@ -384,8 +390,8 @@ def parity_self_check(N, rank, world):
         ls = ds(tids, labels=tids)
         ls.loss.backward()
         # this rank's gradients == the same layers' gradients of the single-stage run (same kernels, same shapes): weight
-        # matrices bit for bit (one GEMM each); norm gains / biases are summed over row blocks with fp32 atomics, whose
-        # order varies from run to run, so those are compared to 2e-3
+        # matrices bit for bit (one GEMM each); norm gains / biases are fp32 sums over row blocks, and the
+        # pipeline's micro-batch split groups the rows differently, so those are compared to 2e-3
         gp, gs = dt.stage.params.hf_state_dict(grads=True), ds.stage.params.hf_state_dict(grads=True)
 
         def same(k, a, b):
@@ -418,6 +424,19 @@ def parity_self_check(N, rank, world):
     torch.cuda.empty_cache()
     return res
 
+
+
+def sample_tensors(sd, per_tensor=4096, seed=1234):
+    """A fixed, seeded sample of every tensor of a state dict (sorted by name), as one float64 array."""
+    import numpy as np
+    import torch
+    out = []
+    for k in sorted(sd):
+        v = sd[k].detach().reshape(-1)
+        g = torch.Generator().manual_seed(seed)
+        idx = torch.randperm(v.numel(), generator=g)[:per_tensor].to(v.device)
+        out.append(v[idx].double().cpu().numpy())
+    return np.concatenate(out)
 
 
 def measure_training(args, N, rank, world, tf_peak, peak_kind):
@@ -465,6 +484,9 @@ def measure_training(args, N, rank, world, tf_peak, peak_kind):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     t = float(t)
+    dump = {"train_loss": [float(loss.detach())]}
+    for grads in (False, True):                    # what the last step left in this rank's parameters and gradients
+        dump["train_grads_sample" if grads else "train_params_sample"] = sample_tensors(dm.stage.params.hf_state_dict(grads=grads))
     tokens = B * S
     flops = 6 * cfg.n_layers * cfg.layer_matmul_params() * tokens + 6 * cfg.vocab * cfg.hidden * tokens \
         + 3 * cfg.n_layers * 2 * B * S * S * cfg.n_heads * cfg.head_dim
@@ -490,8 +512,8 @@ def measure_training(args, N, rank, world, tf_peak, peak_kind):
                                                        "(starting with the lm_head dgrad), then each stage's weight gradients as one GEMM per weight over all micro-batches, "
                                                        "then one fused Adam launch over the stage's arena",
                                            "h2d_bytes_per_step": B * S * 8, "d2h_bytes_per_step": 4},
-           "model_tflops_per_s": flops * args.steps / t / 1e12, "gpu_launches": tr.launches - l0,
-           "roofline": {"bound": "tensor", "kernel": "tcgen05 GEMM (gate/up forward Linear of one layer, timed alone)", "achieved": ach,
+           "model_tflops_per_s": flops * args.steps / t / 1e12, "gpu_launches": tr.launches - l0, "_dump": dump,
+           "roofline": {"bound": "tensor", "kernel": "wgmma GEMM (gate/up forward Linear of one layer, timed alone)", "achieved": ach,
                         "peak": tf_burst, "peak_kind": f"{peak_kind} cuBLAS bf16 (burst: kernel timed alone)", "unit": "TFLOP/s",
                         "frac": ach / tf_burst, "traffic": None, "algorithmic_flops_per_launch": 2.0 * M * Nn * K, "launch_s": tg,
                         "whole_step": {"model_tflops_per_s": flops * args.steps / t / 1e12,
@@ -520,14 +542,20 @@ def main():
     ap.add_argument("--prompt", type=int, default=0, help="override the workload's prompt length")
     ap.add_argument("--new", type=int, default=0, help="override the workload's number of generated tokens")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's outputs as DIR/<name>.npy (float64)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-train", action="store_true", help="skip the secondary training-step measurement")
     ap.add_argument("--no-parity-check", action="store_true", help="skip the tiny-model parity self-check")
-    ap.add_argument("--train-model", default="Qwen/Qwen2.5-7B")
+    # one 80 GB GPU holds a 0.5B model's bf16 weights + gradients + fp32 Adam moments many times over; a 7B one needs
+    # ~92 GB for those alone
+    ap.add_argument("--train-model", default="Qwen/Qwen2.5-0.5B")
     ap.add_argument("--train-batch", type=int, default=8)
     ap.add_argument("--train-seq", type=int, default=512)
     ap.add_argument("--train-mb-per-stage", type=int, default=4, help="micro-batches per pipeline stage in the training step (N > 1)")
     args = ap.parse_args()
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step (--steps >= 1)")
     name, prompt, new, wl_rows = WORKLOADS[args.workload]
     prompt, new = args.prompt or prompt, args.new or new
     args.rows_per_gpu = args.rows_per_gpu or wl_rows
@@ -633,6 +661,7 @@ def main():
     e3.record()
     sync_all()
     t_e2e = torch.tensor([max(e2.elapsed_time(e3) * 1e-3, time.perf_counter() - t0)], device=dm.device)
+    dump = {"tokens": out_host.numpy().astype("float64")}     # what the last timed generate handed to its caller
     clocks = sampler.stop() if rank == 0 else None
     # ---- pipeline occupancy: fraction of the decode phase this rank's compute stream spent inside decode launches
     # (the rest = waiting for a neighbour's activations / ids, i.e. exposed transfer + pipeline bubble)
@@ -658,14 +687,10 @@ def main():
     from tensorlink_b200.ml.shard import gemv_max_rows
     gemv_path = args.rows_per_gpu <= gemv_max_rows()
     tot_b = sum(v["bytes"] for v in gv.values()); tot_s = sum(v["s"] for v in gv.values())
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get(f"gemv_gate_up:{name}")
     roof = {"bound": "hbm", "kernel": ("tl::gemv_stream_kernel (gate/up Linear, RMSNorm prologue + SwiGLU epilogue)" if gemv_path
                                        else "tl::gemm_bf16_kernel (gate/up Linear at M = rows, weight-streaming regime)"),
             "achieved": gv["gate_up"]["GBps"], "peak": hbm_peak, "peak_kind": f"{peak_kind} copy bandwidth (burst)",
-            "unit": "GB/s", "frac": gv["gate_up"]["GBps"] / hbm_peak, "traffic": traffic,
+            "unit": "GB/s", "frac": gv["gate_up"]["GBps"] / hbm_peak, "traffic": None,
             "algorithmic_bytes_per_launch": gv["gate_up"]["bytes"], "launch_s": gv["gate_up"]["s"],
             "all_gemv_launches": {"achieved": tot_b / tot_s / 1e9, "frac": tot_b / tot_s / 1e9 / hbm_peak,
                                   "per_shape_GBps": {k: v["GBps"] for k, v in gv.items()}}}
@@ -711,6 +736,12 @@ def main():
         line["parity_check"] = parity_self_check(N, rank, world)
     if not args.no_train:
         line["train"] = measure_training(args, N, rank, world, tf_peak, peak_kind)
+        dump.update(line["train"].pop("_dump"))
+    if rank == 0 and args.dump_outputs:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for k, v in dump.items():
+            np.save(os.path.join(args.dump_outputs, f"{k}.npy"), np.asarray(v, dtype=np.float64))
     if rank == 0:
         if N == 1 and not args.no_cpu_baseline:
             ref = CpuReference(cfg, rows, prompt, budget_layers=2)

@@ -1,4 +1,4 @@
-/* tensorlink_b200 — C ABI of the B200-native shard executor.
+/* tensorlink_b200 — C ABI of the H100-native shard executor.
  *
  * The reference (tensorlink-lab/tensorlink) has no FFI: its shard operator is Python
  * (`LayerGroupModule.forward(**kwargs)`, tensorlink/ml/injector.py:154-281) and the arithmetic is
@@ -14,7 +14,7 @@
  *  - `stream` is a `cudaStream_t` passed as `void*`; every call is asynchronous on that stream.
  *  - no entry point allocates or frees device memory; workspaces are passed in.
  *  - return value: 0 on success, a negative `tl_status` otherwise; `tl_last_error()` gives the
- *    (thread-local) message.  There is no CPU fallback: on a machine without an sm_100 device
+ *    (thread-local) message.  There is no CPU fallback: on a machine without an sm_90 device
  *    compute calls return TL_ERR_NO_DEVICE.
  *  - rounding points replicate the reference's bf16 pipeline (each HF op output is rounded to bf16
  *    before the next op consumes it); accumulation is fp32.
@@ -35,7 +35,7 @@ typedef enum {
     TL_OK = 0,
     TL_ERR_INVALID = -1,   /* bad shape / alignment / flag combination */
     TL_ERR_CUDA = -2,      /* a CUDA runtime / driver call failed       */
-    TL_ERR_NO_DEVICE = -3, /* no sm_100 device visible                  */
+    TL_ERR_NO_DEVICE = -3, /* no sm_90 device visible                  */
     TL_ERR_WORKSPACE = -4  /* workspace too small                       */
 } tl_status;
 
@@ -60,7 +60,7 @@ int tl_rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd_out, int r
 /* ---- K7  embed_tokens gather (modeling_qwen2.py:367): out[n,:] = table[ids[n],:] */
 int tl_embed_fwd(const int64_t* ids, const void* table, void* out, int n_tokens, int H, int vocab, void* stream);
 
-/* ---- K2/K5/K6/K7  nn.Linear as one tcgen05 GEMM: C[M,N] = A[M,K] * B[N,K]^T (+ epilogue flags above).
+/* ---- K2/K5/K6/K7  nn.Linear as one wgmma GEMM: C[M,N] = A[M,K] * B[N,K]^T (+ epilogue flags above).
  * lda/ldb/ldc in elements.  Replaces q/k/v_proj (modeling_qwen2.py:217-219, fused into one B), o_proj (:244),
  * gate/up/down_proj (:46-48), lm_head (:474-476) and, with the MN-major flags, their dgrad/wgrad. */
 int tl_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,

@@ -7,7 +7,7 @@ installed-HF ``GPT2LMHeadModel`` (124M, seeded random init, fp32, CPU) and the w
 reference's own loop finder cannot split GPT-2 (its ``for i, block in enumerate(self.h)`` is not matched,
 ml/injector.py:75-90; SURVEY.md §8c), so the loop body is handed to LayerGroupModule by hand.  Result: the 2-shard
 output equals the unsharded HF model BIT FOR BIT on CPU — the sharding + codec add no numeric change.  GPT-2 itself is
-not on the B200 path (LayerNorm / GELU / learned positions have no kernels here: config 1 is the reference's CPU
+not on the CUDA path (LayerNorm / GELU / learned positions have no kernels here: config 1 is the reference's CPU
 plumbing case); tests/test_gpt2_plumbing_cpu.py re-runs the same 2-shard composition through THIS repo's wire codec
 (oracle and product) on CPU and checks it against the fixture written here.
 """

@@ -1,2 +1,2 @@
-"""tensorlink_b200 — B200-native shard executor behind tensorlink's DistributedModel API."""
+"""tensorlink_b200 — H100-native shard executor behind tensorlink's DistributedModel API."""
 __version__ = "0.1.0"

@@ -1,7 +1,6 @@
 // Causal GQA attention (SDPA contract: fp32 scores + softmax, P cast to bf16 for P·V, fp32 accumulate).
-//  * prefill / training forward: flash-style, 64-query x 64-key tiles, warp-level mma.sync (round-1 kernel;
-//    the tcgen05/TMEM version is the planned replacement — attention is 3-6 % of the layer FLOPs at the
-//    BASELINE shapes, the tcgen05 GEMMs in gemm.cu carry the rest).
+//  * prefill / training forward: flash-style, 64-query x 64-key tiles, warp-level mma.sync for query runs shorter than
+//    one tile; attention_wgmma.cu serves the rest.
 //  * decode: one query per batch row, split over the KV length, HBM-bound on the cache read.
 #include <stdlib.h>
 
@@ -345,8 +344,7 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(const bf
 
 // ---- split phase on tensor cores (mma.sync m16n8k16).  The n_rep query heads that share a kv head are the M rows of
 // the MMA (16 rows, the unused ones zero): per cached key the CUDA-core kernel above spends 2 * n_rep * D FMAs plus the
-// bf16 unpacking, which at n_rep = 7 is more issue bandwidth than an SM has at its share of the HBM rate (ncu, round 2:
-// 56 us per layer for 67 MB of KV at B = 32, T = 1026 = 1.2 TB/s).  Here a CTA stages its DEC_CHUNK keys and values in
+// bf16 unpacking, which at n_rep = 7 is more issue bandwidth than an SM has at its share of the HBM rate.  Here a CTA stages its DEC_CHUNK keys and values in
 // shared memory with cp.async (coalesced 16-byte pieces, a ring of two 64-key tiles: the next tile is in flight while one
 // is used; DEC_CHUNK_MMA = 256 keys per CTA), each of the 4 warps owns 16 keys of every 64-key tile with its own online-softmax state, and the 4 states are merged
 // through shared memory into the (m, l, o) record the reduce kernel below expects.
@@ -539,10 +537,8 @@ __global__ void attn_decode_reduce_kernel(const float* __restrict__ ws, bf16* __
 }  // namespace tl
 
 namespace tl {
-int attn_prefill_tc_dispatch(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B, int S,
-                             int past_len, int n_h, int n_kv, int d, int T_max, float scale, cudaStream_t st);
-int attn_prefill_tc2_dispatch(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B, int S,
-                              int past_len, int n_h, int n_kv, int d, int T_max, float scale, cudaStream_t st);
+int attn_prefill_wgmma(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B, int S, int past_len,
+                       int n_h, int n_kv, int d, int T_max, float scale, cudaStream_t st);
 }
 
 extern "C" {
@@ -556,19 +552,11 @@ int tl_attn_prefill_fwd(const void* q, const void* k_cache, const void* v_cache,
                "tl_attn_prefill_fwd: past_len %d + S %d exceeds cache T_max %d", past_len, S, T_max);
     if (B == 0 || S == 0) return TL_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    {   // tcgen05 tiles (attention_tc.cu) from one full 128-row query tile upwards; TL_ATTN_IMPL=mma|tc forces a path.
-        // Round-1 measurement (TFLOP/s: mma.sync / first tcgen05 form / second form with O accumulated in TMEM):
-        // d=128: B=8 S=512 156 / 177 / 295, B=16 S=1024 217 / 298 / 532, B=1 S=4096 219 / 319 / 578;
-        // d=64:  B=8 S=512 122 / 127 / 141.
+    {   // wgmma kernel (attention_wgmma.cu) from one full 64-row query tile upwards; TL_ATTN_IMPL=mma|wgmma forces a path
         const char* e = getenv("TL_ATTN_IMPL");          // read per call: tests flip it
-        const int impl = !e ? 0 : (e[0] == 'm' ? 1 : (e[0] == 't' ? 2 : 0));
-        if (impl == 2 || (impl == 0 && S >= 128)) {
-            const char* v = getenv("TL_ATTN_TC");                // 2 (default): O accumulated in TMEM; 1: first form
-            const int rc = (v && v[0] == '1')
-                ? attn_prefill_tc_dispatch(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, T_max, scale, st)
-                : attn_prefill_tc2_dispatch(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, T_max, scale, st);
-            if (rc != 1) return rc;
-        }
+        const int impl = !e ? 0 : (e[0] == 'm' ? 1 : (e[0] == 'w' ? 2 : 0));
+        if (impl == 2 || (impl == 0 && S >= FA_BQ))
+            return attn_prefill_wgmma(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, T_max, scale, st);
     }
     const dim3 grid((S + FA_BQ - 1) / FA_BQ, n_h, B);
     const float sl2 = scale * 1.4426950408889634f;
@@ -828,8 +816,7 @@ extern "C" int tl_attn_decode_fused(const void* qkv, void* k_cache, void* v_cach
     if (use_pdl < 0) {
         const char* e = getenv("TL_PDL");
         const char* e2 = getenv("TL_PDL_ATTN");
-        // measured (round 1, Qwen2.5-7B B=1): an early-resident attention grid costs more than it hides (329 vs 349 tok/s),
-        // so the attribute is opt-in here (TL_PDL_ATTN=1); the weight-streaming Linears keep it on by default
+        // an early-resident attention grid competes with the Linear it overlaps for SMs, so the attribute is opt-in here (TL_PDL_ATTN=1); the weight-streaming Linears keep it on by default
         use_pdl = (!(e && e[0] == '0') && (e2 && e2[0] == '1')) ? 1 : 0;
     }
     cfg.attrs = attr;

@@ -2,7 +2,7 @@
 //   pass 0  D[b,h,s]   = sum_d dO * O                                   (fp32)
 //   pass 1  dQ tile    = sum_kv  dS · K          dS = P ∘ (dO·V^T − D) · scale      (parallel over query tiles)
 //   pass 2  dK,dV tile = sum_{q heads of the group, q tiles}  dS^T · Q ,  P^T · dO   (parallel over key tiles)
-// Warp-level mma.sync like the forward (attention is 3-6 % of the layer FLOPs at the BASELINE shapes).
+// Warp-level mma.sync kernels for sequences shorter than one 64-row tile; attention_wgmma.cu serves the rest.
 // q/o/do/dq: [B,S,n_h,d] token-major;  k/v: [B,n_kv,T_max,d];  dk/dv: [B,n_h,T_max,d] (one partial per query head);
 // lse/D: [B,n_h,S].
 #include <stdlib.h>
@@ -333,9 +333,8 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dkv_kernel(const bf16* __
 }  // namespace tl
 
 namespace tl {
-int attn_bwd_tc_dispatch(const void* q, const void* k_cache, const void* v_cache, const void* dout, const float* lse, const float* Dv,
-                         void* dq, void* dk, void* dv, int B, int S, int n_h, int n_kv, int d, int T_max, float scale,
-                         cudaStream_t st);
+int attn_bwd_wgmma(const void* q, const void* k_cache, const void* v_cache, const void* dout, const float* lse, const float* Dv,
+                   void* dq, void* dk, void* dv, int B, int S, int n_h, int n_kv, int d, int T_max, float scale, cudaStream_t st);
 }
 
 extern "C" {
@@ -356,13 +355,13 @@ int tl_attn_bwd(const void* q, const void* k_cache, const void* v_cache, const v
     const long long total = (long long)B * S * n_h;
     const int g0 = (int)((total * 32 + 255) / 256);
     const dim3 g1((S + AB_BQ - 1) / AB_BQ, n_h, B), g2((S + AB_BKV - 1) / AB_BKV, n_h, B);
-    {   // tcgen05 kernels (attention_bwd_tc.cu) from one full 128-row tile upwards; TL_ATTN_BWD=mma keeps the kernels below
+    {   // wgmma kernels (attention_wgmma.cu) from one full 64-row tile upwards; TL_ATTN_BWD=mma|wgmma forces a path
         const char* e = getenv("TL_ATTN_BWD");
-        if (S >= 128 && !(e && e[0] == 'm')) {
+        const int impl = !e ? 0 : (e[0] == 'm' ? 1 : (e[0] == 'w' ? 2 : 0));
+        if (impl == 2 || (impl == 0 && S >= AB_BQ)) {
             if (d == 64) attn_bwd_dot_kernel<64><<<g0, 256, 0, st>>>((const bf16*)out, (const bf16*)dout, Dv, S, n_h, total);
             else attn_bwd_dot_kernel<128><<<g0, 256, 0, st>>>((const bf16*)out, (const bf16*)dout, Dv, S, n_h, total);
-            const int rc = attn_bwd_tc_dispatch(q, k_cache, v_cache, dout, lse, Dv, dq, dk, dv, B, S, n_h, n_kv, d, T_max, scale, st);
-            if (rc != 1) return rc;
+            return attn_bwd_wgmma(q, k_cache, v_cache, dout, lse, Dv, dq, dk, dv, B, S, n_h, n_kv, d, T_max, scale, st);
         }
     }
     const size_t sm1 = (size_t)6 * 64 * (d + 8) * sizeof(bf16);

@@ -1,17 +1,19 @@
 #!/usr/bin/env bash
-# Build libtensorlink_b200.so in-tree for sm_100a (the .so travels to the GPU box with the snapshot).
+# Build libtensorlink_b200.so in-tree for sm_90a (H100).
 set -euo pipefail
 here="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 out="$here/libtensorlink_b200.so"
 srcs=("$here"/*.cu)
 objs=()
-mkdir -p "$here/build"
+arch=sm_90a
+objdir="$here/build/$arch"     # objects of another architecture are never relinked
+mkdir -p "$objdir"
 pids=()
 for s in "${srcs[@]}"; do
-  o="$here/build/$(basename "${s%.cu}").o"
+  o="$objdir/$(basename "${s%.cu}").o"
   objs+=("$o")
-  if [[ ! -f "$o" || "$s" -nt "$o" || "$here/common.cuh" -nt "$o" || "$here/../../include/tensorlink_b200.h" -nt "$o" ]]; then
-    nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC \
+  if [[ ! -f "$o" || "$s" -nt "$o" || "${BASH_SOURCE[0]}" -nt "$o" || "$here/common.cuh" -nt "$o" || "$here/gemm_common.cuh" -nt "$o" || "$here/../../include/tensorlink_b200.h" -nt "$o" ]]; then
+    nvcc -gencode arch=compute_90a,code=$arch -O3 -std=c++17 -lineinfo -Xcompiler -fPIC \
          ${TL_NVCC_EXTRA:-} -c "$s" -o "$o" &
     pids+=($!)
   fi

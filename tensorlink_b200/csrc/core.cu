@@ -31,7 +31,7 @@ int sm_count() {
         if (cudaGetDevice(&dev) != cudaSuccess ||
             cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
             cudaGetLastError();
-            return 148;
+            return 132;
         }
         cached = n;
     }
@@ -77,8 +77,8 @@ int tl_device_info(int* sm_count, int* cc_major, int* cc_minor) {
     if (sm_count) *sm_count = p.multiProcessorCount;
     if (cc_major) *cc_major = p.major;
     if (cc_minor) *cc_minor = p.minor;
-    if (p.major != 10) {
-        tl::set_error("device is sm_%d%d; this library is built for sm_100a only", p.major, p.minor);
+    if (p.major != 9 || p.minor != 0) {
+        tl::set_error("device is sm_%d%d; this library is built for sm_90a (H100) only", p.major, p.minor);
         return TL_ERR_NO_DEVICE;
     }
     return TL_OK;

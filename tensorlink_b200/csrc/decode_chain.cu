@@ -2,7 +2,7 @@
 //
 // The per-kernel decode path (gemv_stream.cu + attention.cu) pays, at every launch boundary, the tail of one kernel,
 // the ramp-up of the next and (for the attention launch) a few microseconds in which nothing streams at all: the two
-// small Linears of a layer (qkv 33 MB, o 26 MB at Qwen2.5-7B) ran at 2.1 / 1.8 TB/s for that reason (round 1).
+// small Linears of a layer (qkv 33 MB, o 26 MB at Qwen2.5-7B) lose the most to that.
 // Here one CTA per SM stays resident for a whole decoder layer (or any job list up to DC_MAX_JOBS) and walks it:
 //
 //     ATTN(j)  ->  GEMV o(j) (+residual)  ->  GEMV gate/up(j) (+norm, SwiGLU)  ->  GEMV down(j) (+residual)
@@ -10,8 +10,8 @@
 //
 // * The producer warp streams the weight rows of EVERY GEMV job of the chain, in order, into one shared-memory ring
 //   (cp.async.bulk, mbarrier full/empty) and never waits for a dependency: weights are constant.  While the consumer
-//   warps cross a grid barrier, stage the next input vector or run the attention job, the ring (~160-190 KB per SM,
-//   ~25 MB chip-wide, about 4 us of streaming) fills with the next job's weights.
+//   warps cross a grid barrier, stage the next input vector or run the attention job, the ring (~160-190 KB per SM)
+//   fills with the next job's weights.
 // * A dependency is one counter in global memory: writers publish with red.release.gpu, every CTA's thread 0 polls
 //   with ld.acquire.gpu.  No cooperative-groups grid sync, no per-thread fences.  Every spin gives up after 2 s and
 //   raises an error word instead of hanging the GPU.
@@ -832,7 +832,7 @@ int tl_decode_chain_trace(void* buf, int n_slots) {
 }
 
 size_t tl_decode_chain_ws(int M, int n_h, int n_kv, int d) {
-    // attention partials [M*n_h][cpg][d+4] floats with cpg = CTAs / (n_kv*M) <= 160 / (n_kv*M) on any sm_100 part
+    // attention partials [M*n_h][cpg][d+4] floats with cpg = CTAs / (n_kv*M) <= 160 / (n_kv*M) (160 bounds the SM count of every supported part)
     if (M < 1 || n_h < 1 || n_kv < 1) return 0;
     const int cpg = 160 / (n_kv * M) > 0 ? 160 / (n_kv * M) : 1;
     return (size_t)M * n_h * cpg * (d + 4) * sizeof(float) + 256;
@@ -870,8 +870,7 @@ int tl_decode_chain(const tl_decode_job* jobs, int n_jobs, int M, void* sync_slo
     const size_t xs_bytes = (((size_t)M * k_max * 2) + 127) & ~(size_t)127;
     const size_t attn_bytes = (size_t)DC_ATTN_BYTES;
     const size_t fixed = xs_bytes + attn_bytes + 2 * DC_MAX_STAGES * sizeof(uint64_t);
-    // Ring geometry.  The consumers are the scarce resource (one warp per scheduler cannot hide its own latencies:
-    // measured 97 % busy at 5 warps), so all 8 consumer warps get a slot class of their own: 8 slots (n_stages % NW == 0:
+    // Ring geometry.  The consumers are the scarce resource (one warp per scheduler cannot hide its own latencies), so all 8 consumer warps get a slot class of their own: 8 slots (n_stages % NW == 0:
     // a slot is always drained by the same warp) as large as shared memory allows, capped at 24 KB.  TL_CHAIN_STAGE_KB
     // forces a slot size (then as many slots as fit, NW = the largest divisor-compatible warp count).
     static int forced_kb = -1;
@@ -905,8 +904,8 @@ int tl_decode_chain(const tl_decode_job* jobs, int n_jobs, int M, void* sync_slo
     static int dyn = -1, l2_ahead = -1;
     if (dyn < 0) {
         const char* e = getenv("TL_CHAIN_DYNAMIC");      // 1: units handed out by ticket counters instead of the static split
-        dyn = (e && e[0] == '1') ? 1 : 0;                // (measured worse: a ticket covers NW units, too coarse at the tail)
-        const char* a = getenv("TL_CHAIN_L2_AHEAD_KB");  // L2 prefetch lead per CTA; off: measured 2.4x SLOWER at 192 KB
+        dyn = (e && e[0] == '1') ? 1 : 0;                // (a ticket covers NW units, coarse at the tail)
+        const char* a = getenv("TL_CHAIN_L2_AHEAD_KB");  // L2 prefetch lead per CTA; off by default
         l2_ahead = a ? atoi(a) * 1024 : 0;               // (a prefetch followed closely by the load of the same lines is fetched twice)
         if (l2_ahead < 0) l2_ahead = 0;
     }

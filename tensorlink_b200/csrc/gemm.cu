@@ -1,12 +1,13 @@
-// nn.Linear and its gradients as one persistent, warp-specialised tcgen05 GEMM.
+// nn.Linear and its gradients as one persistent, warp-specialised wgmma GEMM (sm_90a).
 //
-//   C[M,N] (+)= A[M,K] · B[N,K]^T        bf16 operands, fp32 accumulation in TMEM
+//   C[M,N] (+)= A[M,K] · B[N,K]^T        bf16 operands, fp32 accumulation in registers
 //
-// CTA = 6 warps: warp 0 = TMA producer, warp 1 = TMEM owner + single-thread MMA issuer, warps 2..5 = epilogue
-// (TMEM lane quarter = warp_id % 4).  128 x BN output tile, BLOCK_K = 64 (one 128-byte swizzle atom of bf16),
-// STAGES-deep smem ring fed by cp.async.bulk.tensor, two TMEM accumulators so the epilogue of tile i overlaps
-// the MMAs of tile i+1.  Operands may be K-major (row-major [rows, K]) or MN-major (row-major [K, rows]) so the
-// same kernel serves forward (x·W^T), dgrad (dy·W) and wgrad (dy^T·x) without transposes.
+// CTA = 3 warpgroups: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers, each issuing
+// m64nBNk16 wgmma for one 64-row half of the 128 x BN output tile and running its epilogue.  BLOCK_K = 64 (one 128-byte
+// swizzle atom of bf16), STAGES-deep smem ring fed by cp.async.bulk.tensor; the producer runs ahead into the next tile
+// while the consumers run the epilogue of the current one.  Operands may be K-major (row-major [rows, K]) or MN-major
+// (row-major [K, rows], wgmma's transpose bits) so the same kernel serves forward (x·W^T), dgrad (dy·W) and
+// wgrad (dy^T·x) without transposes.
 // Tensor-core roofline: 2*M*N*K flops per launch.
 #include <stdlib.h>
 
@@ -17,7 +18,7 @@
 
 namespace tl {
 
-constexpr int GEMM_THREADS = 192;
+constexpr int GEMM_THREADS = 384;
 
 // ---------------------------------------------------------------------------------------- tensor maps (host)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -94,15 +95,24 @@ int make_tensor_map(CUtensorMap* out, const void* ptr, uint64_t inner, uint64_t 
 }
 
 // ---------------------------------------------------------------------------------------- kernel
+// Accumulators of one consumer warpgroup (64 x BN fp32) are written to a padded fp32 tile in shared memory and read back
+// one row per lane for the shared epilogue; after that read the same bytes serve as the per-warp store staging tiles.
 template <int BN>
 struct GemmCfg {
     static constexpr int A_BYTES = BM * BK * 2;         // 16 KB
-    static constexpr int B_BYTES = BN * BK * 2;         // 16 / 32 KB
+    static constexpr int B_BYTES = BN * BK * 2;         // 4 / 16 KB
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 9);
-    static constexpr int TMEM_COLS = 2 * BN;            // two accumulators (>= 32 columns, power of two)
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + EPI_SMEM_BYTES;
+    static constexpr int STAGES = (BN == 128) ? 4 : 8;
+    static constexpr int ACC_PITCH = BN + 4;            // floats; row-per-lane float4 reads are conflict-free
+    static constexpr int ACC_BYTES = 64 * ACC_PITCH * 4;   // per consumer warpgroup
+    static constexpr int UNITS = BN >= 64 ? 2 * (BN / 64) : 2;   // (row half, 64-column chunk) epilogue units per warpgroup
+    static_assert(UNITS <= 4 && UNITS * EPI_STAGE_BYTES <= ACC_BYTES, "epilogue staging must fit in the accumulator tile");
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * ACC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
+
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 template <int BN, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -112,14 +122,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     using Cfg = GemmCfg<BN>;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+    float* acc_tile = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);   // [2][64][ACC_PITCH]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + 2 * Cfg::ACC_BYTES);
     uint64_t* full_bar = bars;                         // [STAGES]
     uint64_t* empty_bar = bars + Cfg::STAGES;          // [STAGES]
-    uint64_t* tmem_full = bars + 2 * Cfg::STAGES;      // [2]
-    uint64_t* tmem_empty = bars + 2 * Cfg::STAGES + 2; // [2]
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
     // split-K (weight-streaming regime, few output tiles): work item = (tile, k range); partial sums go to an fp32
     // workspace Cv[split][M][N] and a small reduce kernel applies the epilogue
@@ -127,28 +135,20 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int total_tiles = mn_tiles * k_splits;
     const int num_k = (K + BK - 1) / BK;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < Cfg::STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tmem_full[a], 1);
-            mbar_init(&tmem_empty[a], 4);   // one arrive per epilogue warp
+            mbar_init(&empty_bar[s], 8);     // one arrive per consumer warp
         }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_base_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_base_slot;
 
-    if (warp == 0) {
-        // ===================================================================== TMA producer
-        if (lane == 0) {
+    if (wg == 0) {
+        // ===================================================================== TMA producer (one thread)
+        if (threadIdx.x == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
@@ -178,84 +178,94 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================================================================== MMA issuer (one thread)
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc_bf16(BM, BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-                tcgen05_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-                const int ks = t / mn_tiles;
-                const int kb0 = ks * kb_per, kb1 = min(num_k, kb0 + kb_per);
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tcgen05_fence_after();
-                    const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-                    const uint32_t sb = sa + Cfg::A_BYTES;
-                    // K-major: 8-row groups 1024 B apart (SBO), LBO unused(=16 B), k-step = 32 B inside the atom
-                    // MN-major: 64-element MN chunks 8192 B apart (LBO), 8-k groups 1024 B apart (SBO), k-step = 2 KB
-                    const uint64_t da = A_MN ? make_smem_desc_sw128(sa, 8192, 1024) : make_smem_desc_sw128(sa, 16, 1024);
-                    const uint64_t db = B_MN ? make_smem_desc_sw128(sb, 8192, 1024) : make_smem_desc_sw128(sb, 16, 1024);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint64_t ak = da + (uint64_t)((A_MN ? 2048 : 32) * k >> 4);
-                        const uint64_t bk = db + (uint64_t)((B_MN ? 2048 : 32) * k >> 4);
-                        umma_bf16(d_tmem, ak, bk, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&empty_bar[stage]);          // frees the smem slot when these MMAs retire
-                    if (kb == kb1 - 1) umma_commit(&tmem_full[acc]);
-                    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-                }
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else {
-        // ===================================================================== epilogue warps (TMEM -> regs -> HBM)
-        const int quarter = warp & 3;                  // TMEM lanes [32*quarter, 32*quarter+32)
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-            const int ks = t / mn_tiles, tt = t - ks * mn_tiles;
-            const int m0 = (tt % tiles_m) * BM, n0 = (tt / tiles_m) * BN;
-            void* Ct = k_splits > 1 ? (void*)(reinterpret_cast<float*>(Cv) + (size_t)ks * M * N) : Cv;
-            mbar_wait(&tmem_full[acc], acc_phase);
-            tcgen05_fence_after();
-            const int row0 = m0 + quarter * 32;
-            const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN);
-            unsigned char* stg = smem + Cfg::STAGES * Cfg::STAGE_BYTES + 256 + (warp - 2) * EPI_STAGE_BYTES;
-            if (BN >= 64) {
-#pragma unroll 1
-                for (int c = 0; c < BN / 64; ++c) {
-                    uint32_t r0[32], r1[32];
-                    tmem_ld32(taddr + (uint32_t)(c * 64), r0);
-                    tmem_ld32(taddr + (uint32_t)(c * 64 + 32), r1);
-                    tmem_ld_wait();
-                    gemm_epilogue_chunk64(r0, r1, stg, Ct, row0, lane, n0 + c * 64, M, N, ldc, bias, residual, ldr, flags);
-                }
-            } else {      // 32-wide tile: one half chunk
-                uint32_t r0[32], r1[32];
-                tmem_ld32(taddr, r0);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; ++j) r1[j] = 0u;
-                gemm_epilogue_chunk64(r0, r1, stg, Ct, row0, lane, n0, M, N, ldc, bias, residual, ldr, flags, 32);
-            }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
+        return;
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+
+    // ========================================================================= consumers: warpgroup 1 = rows 0..63,
+    // warpgroup 2 = rows 64..127 of the 128 x BN tile; each issues m64nBNk16 wgmma on the shared ring
+    const int cw = wg - 1;                     // consumer warpgroup
+    const int wq = warp & 3;                   // warp within it
+    float* my_acc = acc_tile + cw * 64 * Cfg::ACC_PITCH;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        const int ks = t / mn_tiles, tt = t - ks * mn_tiles;
+        const int m0 = (tt % tiles_m) * BM, n0 = (tt / tiles_m) * BN;
+        const int kb0 = ks * kb_per, kb1 = min(num_k, kb0 + kb_per);
+        const bool active = m0 + 64 * cw < M;  // warpgroup-uniform; rows beyond M are TMA zero-fill, not stored
+        float d[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+        int prev = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            {
+                const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + (uint32_t)(cw * 8192);
+                const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+                // K-major: 8-row groups 1024 B apart (SBO), LBO unused, k-step = 32 B inside the swizzle atom
+                // MN-major: 64-element MN chunks 8192 B apart (LBO), 8-k groups 1024 B apart (SBO), k-step = 2 KB
+                const uint64_t da = A_MN ? make_wgmma_desc_sw128(sa, 8192, 1024) : make_wgmma_desc_sw128(sa, 16, 1024);
+                const uint64_t db = B_MN ? make_wgmma_desc_sw128(sb, 8192, 1024) : make_wgmma_desc_sw128(sb, 16, 1024);
+                wgmma_fence_acc(d);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    const uint64_t ak = da + (uint64_t)((A_MN ? 2048 : 32) * k >> 4);
+                    const uint64_t bk = db + (uint64_t)((B_MN ? 2048 : 32) * k >> 4);
+                    const uint32_t acc = (kb > kb0 || k > 0) ? 1u : 0u;
+                    if constexpr (BN == 128) wgmma_m64n128<A_MN ? 1 : 0, B_MN ? 1 : 0>(*reinterpret_cast<float(*)[64]>(d), ak, bk, acc);
+                    else wgmma_m64n32<A_MN ? 1 : 0, B_MN ? 1 : 0>(*reinterpret_cast<float(*)[16]>(d), ak, bk, acc);
+                }
+                wgmma_commit();
+                wgmma_fence_acc(d);
+                wgmma_wait<1>();                   // the previous stage's MMAs have retired: hand its slot back
+            }
+            if (prev >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            }
+            prev = stage;
+            if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_acc(d);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (!active) continue;                  // no rows of this warpgroup in this tile (warpgroup-uniform)
+
+        // ---- epilogue: fragments -> fp32 tile -> one row per lane -> shared epilogue (bias / SwiGLU / residual / ...)
+#pragma unroll
+        for (int i = 0; i < BN / 2; i += 2) {
+            const int r = 16 * wq + (lane >> 2) + 8 * ((i >> 1) & 1);
+            const int c = 8 * (i >> 2) + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(my_acc + r * Cfg::ACC_PITCH + c) = make_float2(d[i], d[i + 1]);
+        }
+        named_bar_sync(1 + cw, 128);
+        const int rh = wq & 1, ch = wq >> 1;   // this warp's epilogue unit: rows [32*rh, +32), columns [64*ch, +64)
+        const bool has_unit = wq < Cfg::UNITS;
+        uint32_t r0[32], r1[32];
+        if (has_unit) {
+            const float* row = my_acc + (32 * rh + lane) * Cfg::ACC_PITCH + 64 * ch;
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+                const float4 v = *reinterpret_cast<const float4*>(row + j);
+                r0[j] = __float_as_uint(v.x); r0[j + 1] = __float_as_uint(v.y); r0[j + 2] = __float_as_uint(v.z); r0[j + 3] = __float_as_uint(v.w);
+            }
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (BN >= 64) v = *reinterpret_cast<const float4*>(row + 32 + j);
+                r1[j] = __float_as_uint(v.x); r1[j + 1] = __float_as_uint(v.y); r1[j + 2] = __float_as_uint(v.z); r1[j + 3] = __float_as_uint(v.w);
+            }
+        }
+        named_bar_sync(1 + cw, 128);            // the fp32 tile is free: reuse it as the store staging tiles
+        if (has_unit) {
+            void* Ct = k_splits > 1 ? (void*)(reinterpret_cast<float*>(Cv) + (size_t)ks * M * N) : Cv;
+            unsigned char* stg = reinterpret_cast<unsigned char*>(my_acc) + wq * EPI_STAGE_BYTES;
+            gemm_epilogue_chunk64(r0, r1, stg, Ct, m0 + 64 * cw + 32 * rh, lane, n0 + 64 * ch, M, N, ldc, bias, residual, ldr,
+                                  flags, BN >= 64 ? 64 : BN);
+        }
+        named_bar_sync(1 + cw, 128);            // staging reads done before the next tile's fragments land
     }
 }
 
@@ -343,8 +353,7 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, void* __restr
 // split-K reduce + epilogue (bias / residual, bf16 out) + the RMSNorm that follows the Linear, one CTA per row:
 // C[m,:] = bf16(bf16(sum_s ws[s][m][:] + bias) + residual[m,:]);  Hn[m,:] = norm_w * bf16(C[m,:] * rstd(C[m,:])).
 // 512 threads per row: one CTA serves a whole row (the norm needs all of it) and only M <= 128 CTAs exist, so the pass is
-// latency-bound; every thread issues all of its 16 partial loads at once.  (With 128 threads x 4 column groups the fused
-// pass took as long as the two kernels it replaced: 11.4 us vs 5.2 + 6.3 us at 32 x 3584, ncu.)  The sum of squares is
+// latency-bound; every thread issues all of its 16 partial loads at once.  The sum of squares is
 // reduced in a different order than rmsnorm_fwd_kernel's, i.e. Hn may differ from the unfused path in a last bf16 bit.
 constexpr int RN_THREADS = 512;
 constexpr int RN_MAXV = 2;
@@ -434,18 +443,6 @@ splitk_reduce_norm_kernel(const float* __restrict__ ws, bf16* __restrict__ C, in
     }
 }
 
-int gemm2_dispatch(bool a_mn, bool b_mn, const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
-                   const void* bias, const void* residual, int flags, cudaStream_t st);
-
-static bool use_2cta() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("TL_GEMM_IMPL");
-        v = (e && e[0] == '1') ? 0 : 1;      // TL_GEMM_IMPL=1cta forces the single-CTA kernel (A/B tests)
-    }
-    return v == 1;
-}
-
 }  // namespace tl
 
 extern "C" size_t tl_gemm_splitk_ws(int M, int N) { return (size_t)8 * (size_t)(M > 128 ? 0 : M) * (size_t)N * sizeof(float); }
@@ -527,18 +524,8 @@ extern "C" int tl_gemm_bf16(const void* A, const void* B, void* C, int M, int N,
     TL_REQUIRE(lda >= (a_mn ? M : K) && ldb >= (b_mn ? N : K), TL_ERR_INVALID, "tl_gemm_bf16: lda/ldb too small");
     TL_REQUIRE((!a_mn || M % 8 == 0), TL_ERR_INVALID, "tl_gemm_bf16: MN-major A needs M %% 8 == 0");
     cudaStream_t st = (cudaStream_t)stream;
-    // 256x256 tiles on CTA pairs (cta_group::2) when there are enough of them to fill the 74 pairs
-    const long long tiles2 = (long long)((M + 255) / 256) * ((N + 255) / 256);
-    if (use_2cta() && M > 128 && N >= 256 && tiles2 * 3 >= (long long)sm_count())     // >= ~2/3 of the 74 pairs busy
-        return gemm2_dispatch(a_mn, b_mn, A, B, C, M, N, K, lda, ldb, ldc, bias, residual, flags, st);
-    // 128x256 tiles when they still fill the machine, else 128x128
-    const long long tiles256 = (long long)((M + BM - 1) / BM) * ((N + 255) / 256);
-    // single-M-tile problems (batched decode, M <= 128) are weight-streaming: prefer >= 2 tiles per CTA so the
-    // pipeline fill / epilogue of one tile overlaps the stream of the next
-    const bool use256 = (N >= 256) && tiles256 >= (long long)sm_count() * (M <= BM ? 2 : 1);
-    // few rows (M <= 128) and not enough 128-wide tiles to occupy every SM: 32-wide tiles (weight streaming)
+    // few rows (M <= 128) and not enough 128-wide tiles to occupy every SM twice: 32-wide tiles (weight streaming)
     if (M <= BM && !b_mn && (long long)((N + 127) / 128) < 2LL * sm_count() && N % 32 == 0)
         return dispatch_major<32>(a_mn, b_mn, A, B, C, M, N, K, lda, ldb, ldc, bias, residual, flags, st);
-    if (use256) return dispatch_major<256>(a_mn, b_mn, A, B, C, M, N, K, lda, ldb, ldc, bias, residual, flags, st);
     return dispatch_major<128>(a_mn, b_mn, A, B, C, M, N, K, lda, ldb, ldc, bias, residual, flags, st);
 }

@@ -257,8 +257,8 @@ extern "C" int tl_gemv_bf16_pf(const void* x, const void* W, void* y, int M, int
     TL_REQUIRE(!(flags & TL_EPI_RESIDUAL) || residual, TL_ERR_INVALID, "tl_gemv_bf16: RESIDUAL flag without pointer");
     cudaStream_t st = (cudaStream_t)stream;
     if (M >= 2 && use_stream_kernel()) {
-        // 2..8 rows on mma.sync (gemv_mma.cu): correct, but measured SLOWER than the CUDA-core stream kernel in
-        // round 1 (its per-row 1-2 KB bulk copies cap an SM at ~1 copy / 50 ns: 2.7 TB/s vs 3.5-5.9) -> opt-in only.
+        // 2..8 rows on mma.sync (gemv_mma.cu): opt-in; its per-row 1-2 KB bulk copies limit how fast an SM can issue
+        // them, and it has not been compared with the CUDA-core stream kernel on H100.
         const char* e = getenv("TL_GEMV_MMA");
         if (e && e[0] == '1') {
             const int rc = gemv_mma_dispatch(x, W, y, M, N, K, bias, residual, norm_w, eps, flags, st);

@@ -1,7 +1,7 @@
 // Decode-shaped Linear for 2..8 rows: the same persistent bulk-copy weight stream as gemv_stream.cu, but the dot
 // products run on the tensor cores (mma.sync m16n8k16: 16 weight rows x 16 k  times  16 k x 8 batch rows), because at
 // M >= 2 the fp32 FMA + bf16->fp32 conversion work of the CUDA-core kernel (not HBM) becomes the limit
-// (measured 3.0-3.8 TB/s at M = 4 and two passes at M = 8).
+// (and needs two passes at M = 8).
 //
 // Work unit = 16 consecutive weight rows (8 gate/up pairs).  A ring stage holds one K chunk of a unit: 16 row segments
 // copied by cp.async.bulk into a padded pitch (conflict-free ldmatrix).  x (optionally RMS-normalised, HF rounding) is

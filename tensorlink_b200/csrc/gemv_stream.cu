@@ -262,8 +262,8 @@ static int launch_stream(const void* x, const void* W, void* y, int N, int K, co
                          const void* norm_w, float eps, int flags, const void* pf_ptr, size_t pf_bytes, cudaStream_t st) {
     auto kern = gemv_stream_kernel<M>;
     // Two half-size rings per SM (16 consumer warps, finer work split, the next kernel's CTAs become resident as soon as
-    // one of the two exits) when an SM's share of W is small — the latency-bound regime of small models: Qwen2.5-0.5B
-    // decode 1210 -> 1343 tok/s (round 2); one deep ring per SM otherwise (7B: 355.1 vs 354.9 tok/s).
+    // one of the two exits) when an SM's share of W is small — the latency-bound regime of small models; one deep
+    // ring per SM otherwise.  The 128 KB threshold has not been re-chosen by measurement on H100.
     // TL_GEMV_CTAS_PER_SM=1|2 forces either.
     static int forced = -1;
     if (forced < 0) {

@@ -44,13 +44,14 @@ __global__ void swiglu_bwd_kernel(const uint4* __restrict__ gu, const uint2* __r
 }
 
 // ------------------------------------------------------------------------------------------------ RMSNorm backward
-// n = x*rstd, g = dy*w:  dx = rstd * (g - n * mean(g*n)) [+ dx_add];  dw[h] += sum_rows dy*n   (fp32 atomics)
+// n = x*rstd, g = dy*w:  dx = rstd * (g - n * mean(g*n)) [+ dx_add];  dw[h] += sum_rows dy*n
+// (dw: one partial row per CTA in dw_part, summed in CTA order by det_reduce_kernel)
 constexpr int NB_THREADS = 128;
 template <int NB_MAXV>
 __global__ void __launch_bounds__(NB_THREADS) rmsnorm_bwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
                                                                    const bf16* __restrict__ dy, const float* __restrict__ rstd,
                                                                    const bf16* __restrict__ dx_add, bf16* __restrict__ dx,
-                                                                   float* __restrict__ dw_accum, int rows, int H,
+                                                                   float* __restrict__ dw_part, int rows, int H,
                                                                    int rows_per_block) {
     const int nvec = H >> 3;
     float dwl[NB_MAXV][8];
@@ -67,7 +68,7 @@ __global__ void __launch_bounds__(NB_THREADS) rmsnorm_bwd_kernel(const bf16* __r
         wreg[i] = idx < nvec ? reinterpret_cast<const uint4*>(w)[idx] : make_uint4(0, 0, 0, 0);
     }
     // the loads of row r+1 are issued before the two block barriers of row r (the row loop is otherwise one dependent
-    // chain per row: 1.3 TB/s at 4096 x 3584 before this, ncu round 1)
+    // chain per row)
     uint4 xn[NB_MAXV], dn[NB_MAXV], an[NB_MAXV];
     auto fetch = [&](int row) {
         const uint4* xr = reinterpret_cast<const uint4*>(x + (size_t)row * H);
@@ -135,13 +136,14 @@ __global__ void __launch_bounds__(NB_THREADS) rmsnorm_bwd_kernel(const bf16* __r
             }
         }
     }
-    if (dw_accum) {
+    if (dw_part) {
+        float* dst = dw_part + (size_t)blockIdx.x * H;
 #pragma unroll
         for (int i = 0; i < NB_MAXV; ++i) {
             const int idx = threadIdx.x + i * NB_THREADS;
             if (idx < nvec) {
 #pragma unroll
-                for (int j = 0; j < 8; ++j) atomicAdd(&dw_accum[idx * 8 + j], dwl[i][j]);
+                for (int j = 0; j < 8; ++j) dst[idx * 8 + j] = dwl[i][j];
             }
         }
     }
@@ -153,7 +155,7 @@ constexpr int NBW_MAXV = 4;
 __global__ void __launch_bounds__(NB_THREADS) rmsnorm_bwd_warp_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
                                                                         const bf16* __restrict__ dy, const float* __restrict__ rstd,
                                                                         const bf16* __restrict__ dx_add, bf16* __restrict__ dx,
-                                                                        float* __restrict__ dw_accum, int rows, int H) {
+                                                                        float* __restrict__ dw_part, int rows, int H) {
     const int nvec = H >> 3, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int gw = blockIdx.x * (NB_THREADS / 32) + warp, nw = gridDim.x * (NB_THREADS / 32);
     float dwl[NBW_MAXV][8];
@@ -209,7 +211,7 @@ __global__ void __launch_bounds__(NB_THREADS) rmsnorm_bwd_warp_kernel(const bf16
             }
         }
     }
-    if (dw_accum) {
+    if (dw_part) {
         __shared__ float sdw[NB_THREADS / 32][NBW_MAXV * 32 * 8 + 1];
 #pragma unroll
         for (int i = 0; i < NBW_MAXV; ++i)
@@ -220,7 +222,7 @@ __global__ void __launch_bounds__(NB_THREADS) rmsnorm_bwd_warp_kernel(const bf16
             float t = 0.f;
 #pragma unroll
             for (int wv = 0; wv < NB_THREADS / 32; ++wv) t += sdw[wv][c];
-            atomicAdd(&dw_accum[c], t);
+            dw_part[(size_t)blockIdx.x * H + c] = t;
         }
     }
 }
@@ -270,17 +272,20 @@ __global__ void __launch_bounds__(128) rope_kv_bwd_kernel(const bf16* __restrict
 // ------------------------------------------------------------------------------------------------ q/k-norm backward
 // Qwen3: q and k heads are RMS-normalised over the head dim before RoPE (modeling_qwen3.py:248-264).  One warp per
 // (token, q-or-k head): recompute rstd from the saved pre-norm qkv, replace the gradient slice of dqkv in place by
-// the gradient w.r.t. the pre-norm vector, accumulate the gain gradients in fp32.
+// the gradient w.r.t. the pre-norm vector, accumulate the gain gradients in fp32: warps stride over the items, and each
+// CTA writes one partial row [q gains | k gains] to part (summed in CTA order by det_reduce_kernel).
 template <int D>
 __global__ void __launch_bounds__(128) qk_norm_bwd_kernel(const bf16* __restrict__ qkv_pre, bf16* __restrict__ dqkv,
                                                            const bf16* __restrict__ qn, const bf16* __restrict__ kn,
-                                                           float* __restrict__ dqn, float* __restrict__ dkn, float eps,
-                                                           int n_tokens, int n_h, int n_kv) {
+                                                           float* __restrict__ part, float eps, int n_tokens, int n_h, int n_kv) {
     constexpr int PER = D / 32;
     const int heads = n_h + 2 * n_kv, nh_qk = n_h + n_kv;
-    const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (gw >= n_tokens * nh_qk) return;
-    const int n = gw / nh_qk, h = gw - n * nh_qk;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float accq[PER], acck[PER];
+#pragma unroll
+    for (int p = 0; p < PER; ++p) accq[p] = acck[p] = 0.f;
+    for (long long item = (long long)blockIdx.x * 4 + warp; item < (long long)n_tokens * nh_qk; item += (long long)gridDim.x * 4) {
+    const int n = (int)(item / nh_qk), h = (int)(item - (long long)n * nh_qk);
     const bool is_q = h < n_h;
     const size_t off = (size_t)n * heads * D + (size_t)h * D;
     const bf16* w = is_q ? qn : kn;
@@ -301,20 +306,31 @@ __global__ void __launch_bounds__(128) qk_norm_bwd_kernel(const bf16* __restrict
         dot += g[p] * x[p] * rstd;
     }
     dot = warp_sum(dot) / (float)D;
-    float* dw = is_q ? dqn : dkn;
 #pragma unroll
     for (int p = 0; p < PER; ++p) {
         const float nrm = x[p] * rstd;
         dqkv[off + lane + 32 * p] = f2bf(rstd * (g[p] - nrm * dot));
-        atomicAdd(&dw[lane + 32 * p], dy[p] * rbf(nrm));
+        if (is_q) accq[p] += dy[p] * rbf(nrm);
+        else acck[p] += dy[p] * rbf(nrm);
     }
+    }
+    __shared__ float sp[4][2 * D];
+#pragma unroll
+    for (int p = 0; p < PER; ++p) {
+        sp[warp][lane + 32 * p] = accq[p];
+        sp[warp][D + lane + 32 * p] = acck[p];
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < 2 * D; c += blockDim.x)
+        part[(size_t)blockIdx.x * 2 * D + c] = sp[0][c] + sp[1][c] + sp[2][c] + sp[3][c];
 }
 
 // ------------------------------------------------------------------------------------------------ cross entropy
-// one CTA per row: loss_sum += logsumexp(row) - row[label]; dlogits = (softmax - onehot) * grad_scale (in place ok)
+// one CTA per row: loss_part[row] = logsumexp(row) - row[label] (0 for ignored rows; summed in row order by
+// det_reduce_kernel); dlogits = (softmax - onehot) * grad_scale (in place ok)
 constexpr int CE_THREADS = 512;
 __global__ void __launch_bounds__(CE_THREADS) ce_fwd_bwd_kernel(const bf16* __restrict__ logits, const int64_t* __restrict__ labels,
-                                                                 float* __restrict__ loss_sum, int32_t* __restrict__ n_valid,
+                                                                 float* __restrict__ loss_part, int32_t* __restrict__ n_valid,
                                                                  bf16* __restrict__ dlogits, float grad_scale, int V) {
     const int row = blockIdx.x;
     const long long label = labels[row];
@@ -324,6 +340,7 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_bwd_kernel(const bf16* __re
     __shared__ float red[CE_THREADS / 32];
     __shared__ float s_bcast;
     if (label < 0 || label >= V) {      // ignore_index (-100): zero gradient, no loss
+        if (threadIdx.x == 0) loss_part[row] = 0.f;
         if (dlogits) for (int i = threadIdx.x; i < nvec; i += CE_THREADS) reinterpret_cast<uint4*>(dr)[i] = make_uint4(0, 0, 0, 0);
         return;
     }
@@ -360,7 +377,7 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_bwd_kernel(const bf16* __re
         for (int i = 0; i < CE_THREADS / 32; ++i) s += red[i];
         s_bcast = s;
         const float lse = mx + logf(s);
-        atomicAdd(loss_sum, lse - bf2f(lr[label]));
+        loss_part[row] = lse - bf2f(lr[label]);
         if (n_valid) atomicAdd(n_valid, 1);
     }
     __syncthreads();
@@ -382,20 +399,35 @@ __global__ void __launch_bounds__(CE_THREADS) ce_fwd_bwd_kernel(const bf16* __re
 }
 
 // ------------------------------------------------------------------------------------------------ embedding backward
+// dtable[ids[t]] += dout[t].  The warp of the FIRST token carrying an id adds the rows of every token with that id, in
+// token order (bf16 rounding after each add), so no two warps touch one table row and the result is the same every run.
 __global__ void embed_bwd_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ dout, bf16* __restrict__ dtable,
                                  int n_tokens, int H, int vocab) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= n_tokens) return;
     const long long id = ids[warp];
     if (id < 0 || id >= vocab) return;
-    const __nv_bfloat162* src = reinterpret_cast<const __nv_bfloat162*>(dout + (size_t)warp * H);
+    for (int j0 = 0; j0 < warp; j0 += 32) {
+        const int j = j0 + lane;
+        if (__any_sync(0xffffffffu, j < warp && ids[j] == id)) return;   // an earlier token owns this row
+    }
     __nv_bfloat162* dst = reinterpret_cast<__nv_bfloat162*>(dtable + (size_t)id * H);
-    for (int i = lane; i < (H >> 1); i += 32) atomicAdd(&dst[i], src[i]);
+    for (int j0 = warp; j0 < n_tokens; j0 += 32) {
+        const int j = j0 + lane;
+        unsigned m = __ballot_sync(0xffffffffu, j < n_tokens && ids[j] == id);
+        while (m) {
+            const int t = j0 + __ffs(m) - 1;
+            m &= m - 1;
+            const __nv_bfloat162* src = reinterpret_cast<const __nv_bfloat162*>(dout + (size_t)t * H);
+            for (int i = lane; i < (H >> 1); i += 32) dst[i] = __hadd2(dst[i], src[i]);
+        }
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ column sum (bias grad)
-// db_accum[c] += sum_m dy[m, c]   (fp32 atomics).  block = 32x8 threads: 64 columns x a 256-row slab
-__global__ void colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ db, int M, int N, int ld) {
+// db_accum[c] += sum_m dy[m, c].  block = 32x8 threads: 64 columns x a 256-row slab; the slab's sums go to row
+// blockIdx.y of part [slabs][N] (summed in slab order by det_reduce_kernel)
+__global__ void colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ part, int M, int N, int ld) {
     const int c2 = blockIdx.x * 32 + threadIdx.x;      // bf16x2 column index
     float a0 = 0.f, a1 = 0.f;
     const int m0 = blockIdx.y * 256, m1 = min(M, m0 + 256);
@@ -413,8 +445,8 @@ __global__ void colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ d
     if (threadIdx.y == 0 && 2 * c2 < N) {
 #pragma unroll
         for (int j = 1; j < 8; ++j) { a0 += s0[j][threadIdx.x]; a1 += s1[j][threadIdx.x]; }
-        atomicAdd(&db[2 * c2], a0);
-        atomicAdd(&db[2 * c2 + 1], a1);
+        part[(size_t)blockIdx.y * N + 2 * c2] = a0;
+        part[(size_t)blockIdx.y * N + 2 * c2 + 1] = a1;
     }
 }
 
@@ -523,6 +555,32 @@ __global__ void adamw_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, f
     }
 }
 
+// acc[c] += sum_b part[b * ld + c] for b = 0..nb-1 in order.  Kernels that reduce over rows write one partial row per
+// CTA instead of adding with float atomics: atomics add in whatever order the CTAs finish, so two runs of one training
+// step would differ in the last bits and, through the optimizer, drift apart.
+__global__ void det_reduce_kernel(const float* __restrict__ part, int nb, int n, int ld, float* __restrict__ acc) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n) return;
+    float s = 0.f;
+    for (int b = 0; b < nb; ++b) s += part[(size_t)b * ld + c];
+    acc[c] += s;
+}
+
+// stream-ordered scratch for the partial rows (the default memory pool keeps it cached)
+static float* det_alloc(size_t floats, cudaStream_t st) {
+    void* p = nullptr;
+    if (cudaMallocAsync(&p, floats * sizeof(float), st) != cudaSuccess) {
+        set_error("stream-ordered allocation of %zu bytes failed", floats * sizeof(float));
+        return nullptr;
+    }
+    return (float*)p;
+}
+static int det_finish(float* part, int nb, int n, int ld, float* acc, cudaStream_t st, const char* what) {
+    det_reduce_kernel<<<(n + 127) / 128, 128, 0, st>>>(part, nb, n, ld, acc);
+    cudaFreeAsync(part, st);
+    return check_launch(what);
+}
+
 static inline int ew_grid(size_t n, int threads) {
     size_t b = (n + threads - 1) / threads;
     const size_t cap = (size_t)sm_count() * 16;
@@ -567,23 +625,29 @@ int tl_rmsnorm_bwd(const void* x, const void* w, const void* dy, const float* rs
     const int grid = (rows + rpb - 1) / rpb;
     const int nv = ((H >> 3) + NB_THREADS - 1) / NB_THREADS;
     cudaStream_t st = (cudaStream_t)stream;
-    if ((H >> 3) <= 32 * NBW_MAXV) {
-        int g = (rows + 3) / 4;
-        const int cap = sm_count() * 4;
-        if (g > cap) g = cap;
+    const bool warp_rows = (H >> 3) <= 32 * NBW_MAXV;
+    int g = (rows + 3) / 4;
+    if (g > sm_count() * 4) g = sm_count() * 4;
+    const int nb = warp_rows ? g : grid;
+    float* part = nullptr;
+    if (dw_accum && !(part = det_alloc((size_t)nb * H, st))) return TL_ERR_CUDA;
+    if (warp_rows) {
         rmsnorm_bwd_warp_kernel<<<g, NB_THREADS, 0, st>>>((const bf16*)x, (const bf16*)w, (const bf16*)dy, rstd,
-                                                          (const bf16*)dx_add, (bf16*)dx, dw_accum, rows, H);
-        return check_launch("tl_rmsnorm_bwd");
-    }
+                                                          (const bf16*)dx_add, (bf16*)dx, part, rows, H);
+    } else {
 #define TL_NB(MV)                                                                                                       \
     rmsnorm_bwd_kernel<MV><<<grid, NB_THREADS, 0, st>>>((const bf16*)x, (const bf16*)w, (const bf16*)dy, rstd,          \
-                                                       (const bf16*)dx_add, (bf16*)dx, dw_accum, rows, H, rpb)
-    if (nv <= 1) TL_NB(1);
-    else if (nv <= 2) TL_NB(2);
-    else if (nv <= 4) TL_NB(4);
-    else TL_NB(8);
+                                                       (const bf16*)dx_add, (bf16*)dx, part, rows, H, rpb)
+        if (nv <= 1) TL_NB(1);
+        else if (nv <= 2) TL_NB(2);
+        else if (nv <= 4) TL_NB(4);
+        else TL_NB(8);
 #undef TL_NB
-    return check_launch("tl_rmsnorm_bwd");
+    }
+    if (!part) return check_launch("tl_rmsnorm_bwd");
+    const int rc = check_launch("tl_rmsnorm_bwd");
+    if (rc != TL_OK) { cudaFreeAsync(part, st); return rc; }
+    return det_finish(part, nb, H, H, dw_accum, st, "tl_rmsnorm_bwd (dw reduce)");
 }
 
 int tl_rope_kv_bwd(const void* dq, const void* dk, const void* dv, void* dqkv, const void* cos_tab, const void* sin_tab,
@@ -609,15 +673,22 @@ int tl_qk_norm_bwd(const void* qkv_pre, void* dqkv, const void* q_norm_w, const 
     TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "tl_qk_norm_bwd: head_dim %d not in {64,128}", d);
     if (n_tokens == 0) return TL_OK;
     const long long warps = (long long)n_tokens * (n_h + n_kv);
-    const int grid = (int)((warps + 3) / 4);
+    long long g = (warps + 3) / 4;
+    if (g > sm_count() * 4) g = sm_count() * 4;
+    const int grid = (int)g;
     cudaStream_t st = (cudaStream_t)stream;
+    float* part = det_alloc((size_t)grid * 2 * d, st);
+    if (!part) return TL_ERR_CUDA;
     if (d == 64)
         qk_norm_bwd_kernel<64><<<grid, 128, 0, st>>>((const bf16*)qkv_pre, (bf16*)dqkv, (const bf16*)q_norm_w, (const bf16*)k_norm_w,
-                                                     dqn_accum, dkn_accum, eps, n_tokens, n_h, n_kv);
+                                                     part, eps, n_tokens, n_h, n_kv);
     else
         qk_norm_bwd_kernel<128><<<grid, 128, 0, st>>>((const bf16*)qkv_pre, (bf16*)dqkv, (const bf16*)q_norm_w, (const bf16*)k_norm_w,
-                                                      dqn_accum, dkn_accum, eps, n_tokens, n_h, n_kv);
-    return check_launch("tl_qk_norm_bwd");
+                                                      part, eps, n_tokens, n_h, n_kv);
+    int rc = check_launch("tl_qk_norm_bwd");
+    if (rc != TL_OK) { cudaFreeAsync(part, st); return rc; }
+    det_reduce_kernel<<<(d + 127) / 128, 128, 0, st>>>(part + d, grid, d, 2 * d, dkn_accum);
+    return det_finish(part, grid, d, 2 * d, dqn_accum, st, "tl_qk_norm_bwd (gain reduce)");   // frees part
 }
 
 int tl_ce_fwd_bwd(const void* logits, const int64_t* labels, float* loss_sum, int32_t* n_valid, void* dlogits,
@@ -625,9 +696,13 @@ int tl_ce_fwd_bwd(const void* logits, const int64_t* labels, float* loss_sum, in
     using namespace tl;
     TL_REQUIRE(V % 8 == 0, TL_ERR_INVALID, "tl_ce_fwd_bwd: V %% 8 != 0");
     if (M == 0) return TL_OK;
-    ce_fwd_bwd_kernel<<<M, CE_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, labels, loss_sum, n_valid, (bf16*)dlogits,
-                                                                  grad_scale, V);
-    return check_launch("tl_ce_fwd_bwd");
+    cudaStream_t st = (cudaStream_t)stream;
+    float* part = det_alloc((size_t)M, st);
+    if (!part) return TL_ERR_CUDA;
+    ce_fwd_bwd_kernel<<<M, CE_THREADS, 0, st>>>((const bf16*)logits, labels, part, n_valid, (bf16*)dlogits, grad_scale, V);
+    const int rc = check_launch("tl_ce_fwd_bwd");
+    if (rc != TL_OK) { cudaFreeAsync(part, st); return rc; }
+    return det_finish(part, M, 1, 1, loss_sum, st, "tl_ce_fwd_bwd (loss reduce)");
 }
 
 int tl_embed_bwd(const int64_t* ids, const void* dout, void* dtable, int n_tokens, int H, int vocab, void* stream) {
@@ -643,8 +718,13 @@ int tl_colsum(const void* dy, float* db_accum, int M, int N, int ld, void* strea
     TL_REQUIRE(N % 2 == 0 && ld % 2 == 0, TL_ERR_INVALID, "tl_colsum: N/ld must be even");
     if (M == 0) return TL_OK;
     const dim3 grid((N / 2 + 31) / 32, (M + 255) / 256), block(32, 8);
-    colsum_kernel<<<grid, block, 0, (cudaStream_t)stream>>>((const bf16*)dy, db_accum, M, N, ld);
-    return check_launch("tl_colsum");
+    cudaStream_t st = (cudaStream_t)stream;
+    float* part = det_alloc((size_t)grid.y * N, st);
+    if (!part) return TL_ERR_CUDA;
+    colsum_kernel<<<grid, block, 0, st>>>((const bf16*)dy, part, M, N, ld);
+    const int rc = check_launch("tl_colsum");
+    if (rc != TL_OK) { cudaFreeAsync(part, st); return rc; }
+    return det_finish(part, (int)grid.y, N, N, db_accum, st, "tl_colsum (reduce)");
 }
 
 int tl_f32_to_bf16_accum(const float* src, void* dst, size_t n, int accumulate, void* stream) {
@@ -687,7 +767,7 @@ int tl_adamw_step(void* param, const void* grad, float* exp_avg, float* exp_avg_
                "tl_adamw_step: arenas must be 16-byte aligned");
     const float bc1 = 1.0f - powf(beta1, (float)step);
     const float bc2s = sqrtf(1.0f - powf(beta2, (float)step));
-    // evict-first loads / stores: 6.17 vs 6.13 TB/s over a 2e9-parameter arena (0.95 of the measured copy peak); TL_ADAM_STREAM=0 = plain
+    // evict-first loads / stores (the arena is touched once per step); TL_ADAM_STREAM=0 = plain
     static int stream_hint = -1;
     if (stream_hint < 0) {
         const char* e = getenv("TL_ADAM_STREAM");

@@ -1,4 +1,4 @@
-"""``DistributedModel`` — the reference's user-facing front end, driving B200 pipeline stages.
+"""``DistributedModel`` — the reference's user-facing front end, driving H100 pipeline stages.
 
 Mirrors /root/reference/tensorlink/ml/module.py: constructor signature (:251-265), ``forward`` returning an HF-style
 output with ``.logits`` / ``.loss`` (:348-407), ``generate`` (:763-769), ``create_optimizer`` (:1016-1021),
@@ -8,7 +8,7 @@ process on one GPU (``torchrun``), all of them construct the same ``DistributedM
 go stage -> stage directly over NVLink (p2p/link.py).  With one process the whole model is a single stage.
 
 Documented deviations from the reference: errors raise instead of being swallowed into ``{"error": ...}`` dicts
-(module.py:978-985); ``dtype`` defaults to bf16 (the only dtype the sm_100a kernels implement); logits live on
+(module.py:978-985); ``dtype`` defaults to bf16 (the only dtype the sm_90a kernels implement); logits live on
 the last stage (pass ``gather_logits=True`` to copy them to rank 0).
 """
 from __future__ import annotations
@@ -66,7 +66,7 @@ def _check_unconsumed(kwargs: dict, what: str):
     for k, v in kwargs.items():
         ok = _NEUTRAL_KW.get(k)
         if ok is None or not any(v is o or (o is not None and v == o) for o in ok):
-            raise NotImplementedError(f"{what}: keyword {k}={v!r} is not supported by the B200 stage executor "
+            raise NotImplementedError(f"{what}: keyword {k}={v!r} is not supported by the H100 stage executor "
                                       "(it would be silently ignored otherwise)")
 
 

@@ -1,4 +1,4 @@
-"""The CUDA shard operator: a contiguous layer range executed by the sm_100a kernels.
+"""The CUDA shard operator: a contiguous layer range executed by the sm_90a kernels.
 
 Mirrors the reference's shard operator ``LayerGroupModule`` (/root/reference/tensorlink/ml/injector.py:154-281):
 same constructor role (a list of layers + the loop live-ins), ``num_layers`` attribute, ``forward(**kwargs) ->
@@ -32,10 +32,9 @@ _GEMV_MAX_ROWS = None
 
 
 def gemv_max_rows() -> int:
-    """Rows per decode step up to which the weight-streaming GEMV path is used; more rows go through the tcgen05 GEMM
+    """Rows per decode step up to which the weight-streaming GEMV path is used; more rows go through the wgmma GEMM
     path (one weight pass for all rows; the GEMV kernel needs a second pass above 4 rows and spends CUDA-core FMAs per
-    row).  Measured on Qwen2.5-7B (tok/s, GEMV vs GEMM path): 3 rows 802 / 667, 4 rows 851 / 929, 8 rows 880 / 1783 ->
-    default 3.  TL_GEMV_MAX_ROWS overrides (1..8)."""
+    row).  Default 3, not yet re-chosen by measurement on H100; TL_GEMV_MAX_ROWS overrides (1..8)."""
     global _GEMV_MAX_ROWS
     if _GEMV_MAX_ROWS is None:
         import os
@@ -195,7 +194,7 @@ class ShardBuffers:
 
 
 class CudaLayerGroup:
-    """B200 shard operator (LayerGroupModule mirror, injector.py:154-281)."""
+    """CUDA shard operator (LayerGroupModule mirror, injector.py:154-281)."""
 
     def __init__(self, cfg: ShardModelConfig, params: ShardParams, max_batch: int, max_seq: int,
                  max_tokens: Optional[int] = None):
@@ -308,7 +307,7 @@ class CudaLayerGroup:
         nat.gemv(w.act, v[f"l{li}.wd"], out=x if out is None else out, residual=x, next_w=after)
 
     def _layer_decode_batched(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor] = None):
-        """More single-token rows than the GEMV path takes: tcgen05 GEMMs in the weight-streaming regime (split along K
+        """More single-token rows than the GEMV path takes: wgmma GEMMs in the weight-streaming regime (split along K
         where a Linear has too few output tiles to occupy every SM) + decode attention.  The RMSNorm after each
         residual Linear rides in that Linear's split-K reduce pass, so layer j > 0 finds its normalised input in w.h."""
         cfg, v, li = self.cfg, self.p.v, self.layer_ids[j]
@@ -367,11 +366,9 @@ class CudaLayerGroup:
 
     # ------------------------------------------------------------------------------------------ chained decode step
     def chain_ok(self, B: int) -> bool:
-        """Rows / shapes the persistent chain kernel (csrc/decode_chain.cu) takes.  Opt-in (TL_DECODE_IMPL=chain): measured
-        on Qwen2.5-7B it streams every Linear at the HBM rate (the GEMV phases of a layer sum to 69-75 us against a 72 us
-        bound) but pays 6-7 us per software dependency (release/acquire counter + restaging the input vector) where a
-        programmatic-dependent-launch boundary costs ~4 us: 323 tok/s against 355+ for the per-kernel sequence
-        (profiles/r02_decode_chain_timeline.txt)."""
+        """Rows / shapes the persistent chain kernel (csrc/decode_chain.cu) takes.  Opt-in (TL_DECODE_IMPL=chain): it streams every Linear at
+        the HBM rate but pays a software dependency (release/acquire counter + restaging the input vector) per phase where
+        the default per-kernel sequence pays a programmatic-dependent-launch boundary."""
         import os
         cfg = self.cfg
         return (os.environ.get("TL_DECODE_IMPL", "kernels") == "chain" and self.allow_chain and self.num_layers > 0

@@ -1,4 +1,4 @@
-"""One pipeline stage on one B200: parameters + per-micro-batch shard operators + captured decode graphs.
+"""One pipeline stage on one H100: parameters + per-micro-batch shard operators + captured decode graphs.
 
 This is the worker half of the reference's hot path (/root/reference/tensorlink/ml/worker.py):
 ``load_module`` (:452-505) -> ``CudaStage.__init__``; ``_handle_forward`` (:297-357) -> ``prefill`` / ``decode``;

@@ -8,7 +8,7 @@ Reference semantics being replaced (/root/reference/tensorlink/ml):
     autograd graph, returning the gradient of the shard input (worker.py:233-295, zeros where a grad is missing);
   * ``optimizer.step()`` / ``zero_grad()`` fan out to every worker (optim.py:131-187, worker.py:1309-1327).
 Here each rank owns its stage's flat parameter and gradient arenas; the backward of a decoder layer is eight
-tcgen05 GEMMs (dgrad + wgrad, MN-major operands, gradient accumulation in the epilogue) plus the attention /
+wgmma GEMMs (dgrad + wgrad, MN-major operands, gradient accumulation in the epilogue) plus the attention /
 norm / RoPE / SwiGLU backward kernels; gradients of ``hidden_states`` hop rank i+1 -> i over NVLink.  The loss and
 its gradient are produced on the last stage by a fused lm_head + cross-entropy pass over token chunks, so the
 [tokens, vocab] logits never exist in full (one micro-batch); in a pipelined step only logits + loss run in the forward

@@ -1,4 +1,4 @@
-"""``DistributedWorker`` — the reference's worker-side shard executor surface over the B200 stage.
+"""``DistributedWorker`` — the reference's worker-side shard executor surface over the H100 stage.
 
 Mirrors the handler names and argument meaning of /root/reference/tensorlink/ml/worker.py so that code written
 against the reference's worker (its network process, or tests that drive a worker directly) can hold this object:

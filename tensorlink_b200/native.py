@@ -1,6 +1,6 @@
 """ctypes binding of ``libtensorlink_b200.so`` (the C ABI in ``include/tensorlink_b200.h``).
 
-There is no CPU fallback and no eager-PyTorch twin: if the library is missing, or no sm_100 device is
+There is no CPU fallback and no eager-PyTorch twin: if the library is missing, or no sm_90 (H100) device is
 visible, every compute entry point raises.  PyTorch is used only to own device memory and streams.
 """
 from __future__ import annotations
@@ -141,12 +141,12 @@ _device_ok = False
 
 
 def require_device():
-    """Raise unless a B200-class (sm_100) device is current."""
+    """Raise unless an H100-class (sm_90) device is current."""
     global _device_ok
     if _device_ok:
         return
     if not torch.cuda.is_available():
-        raise NativeError("no CUDA device: the tensorlink_b200 shard executor runs on sm_100a only")
+        raise NativeError("no CUDA device: the tensorlink_b200 shard executor runs on sm_90a only")
     sm, ma, mi = c_int(), c_int(), c_int()
     _check(load().tl_device_info(sm, ma, mi), "tl_device_info")
     _device_ok = True
@@ -244,7 +244,7 @@ _PREFETCH_BYTES = None
 
 
 def prefetch_bytes() -> int:
-    """How much of the next launch's weights a GEMV asks L2 to fetch (TL_PREFETCH_MB, default 8 — measured best of 0/8/32/64: 349.0 / 355.6 / 352.1 / 351.7 tok/s; 0 disables)."""
+    """How much of the next launch's weights a GEMV asks L2 to fetch (TL_PREFETCH_MB, default 8; 0 disables).  The default has not been re-chosen by measurement on H100."""
     global _PREFETCH_BYTES
     if _PREFETCH_BYTES is None:
         _PREFETCH_BYTES = int(float(os.environ.get("TL_PREFETCH_MB", "8")) * (1 << 20))

@@ -1,4 +1,4 @@
-"""``Torchnode``-shaped packet adapter: a B200 stage behind the reference's FORWARD / BACKWARD packets (SURVEY.md §8 f-4).
+"""``Torchnode``-shaped packet adapter: an H100 stage behind the reference's FORWARD / BACKWARD packets (SURVEY.md §8 f-4).
 
 What the reference's network process does for the hot path (/root/reference/tensorlink/p2p/torch_node.py):
 

@@ -1,4 +1,4 @@
-"""The reference's wire format for shard calls, so that a B200 stage can sit behind an unmodified reference peer
+"""The reference's wire format for shard calls, so that an H100 stage can sit behind an unmodified reference peer
 (SURVEY.md §8 f-4).  Payload level only: sockets, packet prefixes and the DHT stay on the reference side.
 
 Frame (what `tensor_to_bytes` / `bytes_to_tensor` exchange, /root/reference/tensorlink/ml/utils.py:569-660):

@@ -1,4 +1,4 @@
-"""Run under torchrun with one B200 per rank (NCCL): pipeline-sharded results must equal the single-stage results
+"""Run under torchrun with one H100 per rank (NCCL): pipeline-sharded results must equal the single-stage results
 computed with the same kernels on rank 0's GPU (sharding must not change a bit: same launches, same order)."""
 import os
 import sys

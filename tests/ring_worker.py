@@ -1,4 +1,4 @@
-"""Run under torchrun, one B200 per rank, any world size <= n_layers: greedy generation through a world-stage pipeline
+"""Run under torchrun, one H100 per rank, any world size <= n_layers: greedy generation through a world-stage pipeline
 with the decode hops on peer-mapped mailboxes must equal the NCCL send/recv path and the single-stage run."""
 import os
 import sys

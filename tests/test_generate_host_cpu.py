@@ -60,7 +60,7 @@ def _pipeline_model():
 
 
 def test_timeline_model_reproduces_the_measured_schedules():
-    """tools/pipeline_model.py against the step times measured on B200s (DESIGN.md §5, profiles/r02_pipeline_schedule.txt):
+    """tools/pipeline_model.py against fixed schedule step times (a regression fixture for the model, DESIGN.md §5):
     one unit ~ 1 ms at 2 micro-batches per stage; the split head is what the model said it would be worth."""
     pm = _pipeline_model()
     measured_fused = {2: ([15, 13], 232.0), 4: ([8, 8, 8, 4], 267.0), 8: ([4, 4, 4, 4, 4, 4, 3, 1], 309.0)}

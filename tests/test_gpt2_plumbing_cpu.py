@@ -1,5 +1,5 @@
 """BASELINE config 1: GPT-2 small (124M), 2 CPU shards (blocks 0-5 / 6-11), one forward on (1,128) synthetic tokens —
-the reference's *plumbing* case (no GPU, no B200 kernels involved).
+the reference's *plumbing* case (no GPU, no CUDA kernels involved).
 
 The fixture (tests/golden/ref_gpt2_2shards.pt, oracle/gen_golden_gpt2.py) was produced by the reference's own
 ``LayerGroupModule`` + wire codec and equals the unsharded HF model bit for bit.  Here the same two-shard composition

@@ -126,7 +126,7 @@ def test_generate_teacher_forced_exact(cfg):
 
 
 def test_batched_decode_gemm_path():
-    """B = 16 rows decode through the tcgen05 GEMM path; rows are independent, so row i must equal a B=1 run."""
+    """B = 16 rows decode through the wgmma GEMM path; rows are independent, so row i must equal a B=1 run."""
     cfg = C.TINY_QWEN2_D128
     ids = synthetic_tokens(cfg, 16, 10)
     big = make(cfg, max_batch=16).generate(ids, max_new_tokens=12).cpu()
@@ -185,7 +185,7 @@ def test_long_context_decode_consistency(max_seq):
 
 
 def test_batch32_decode_rows_independent():
-    """BASELINE config 5 batch (32 rows per step, tcgen05 GEMM + split-K decode path) at full 0.5B width: every row
+    """BASELINE config 5 batch (32 rows per step, wgmma GEMM + split-K decode path) at full 0.5B width: every row
     of the batched generation equals the same prompt generated alone (B = 1, GEMV path) wherever the one-shot top-2
     margin is resolvable."""
     cfg = C.QWEN25_05B

@@ -3,7 +3,7 @@ vectors the reference's own ``LayerGroupModule`` produced.
 
   (a) full-size Qwen2.5-0.5B (BASELINE config 2): logits of a 32-token prompt and greedy ids, same seeded weights;
   (b) one decoder layer at Qwen2.5-7B width and one at Qwen3-8B width + the full-vocabulary lm_head: a 192-token
-      prefill (tcgen05 GEMMs incl. the 2-CTA form, tcgen05 attention), then 4 single-token decode steps through the
+      prefill (wgmma GEMMs, wgmma attention), then 4 single-token decode steps through the
       weight-streaming GEMV path with the fused (T_max <= 2048) and the split-KV (T_max = 4096) decode attention;
   (c) the CUDA shard operator teacher-forced on ``tests/golden/ref_layergroup_*.pt`` hop by hop.
 
@@ -98,7 +98,7 @@ def test_full_width_layer_and_head_vs_oracle(base, max_seq):
         tail = slice(S - 8, S)
         l16 = F.linear(O.rmsnorm(h16[:, tail], m16.norm, cfg.rms_eps), m16.head)
         l32 = F.linear(O.rmsnorm(h32[:, tail], m32.norm, cfg.rms_eps), m32.head)
-    # ---- prefill through the product path (tcgen05 GEMMs + tcgen05 attention), logits through head_logits
+    # ---- prefill through the product path (wgmma GEMMs + wgmma attention), logits through head_logits
     x = st.prefill(st.embed(ids.cuda()), 0, 0)
     _chain(f"{cfg.name} layer output [1,{S},H]", x.cpu(), h16, h32)
     got = st.head_logits(x[0, tail].contiguous()).cpu()[None]
@@ -163,7 +163,7 @@ def _oracle_grads(cfg, sd0, ids, dtype):
 @pytest.mark.parametrize("base", [C.QWEN25_7B, C.QWEN3_8B], ids=lambda c: c.name)
 @pytest.mark.parametrize("n_mb", [1, 2], ids=["fused-head", "split-head-deferred-w"])
 def test_full_width_training_step_vs_oracle_autograd(base, n_mb):
-    """One optimizer step's worth of gradients through a full-width decoder layer and the 152k-row lm_head (tcgen05
+    """One optimizer step's worth of gradients through a full-width decoder layer and the 152k-row lm_head (wgmma
     GEMMs with MN-major operands at the real K / N, attention backward at 28/4 and 32/8 heads of 128, fused CE over the
     real vocabulary) against the oracle's autograd in fp32; the oracle's own bf16 run sets the yardstick.  n_mb = 2 runs
     the pipelined form: deferred weight gradients and the split head backward (ml/train.py)."""

@@ -82,13 +82,14 @@ def test_rope_kv_bwd(nat, cfg):
     assert O.rel_l2(got[:, :, n_h + n_kv:].transpose(1, 2), dv) <= TOL
 
 
-@pytest.mark.parametrize("B,S,n_h,n_kv,d,impl", [
-    (2, 64, 4, 2, 64, "mma"), (1, 100, 14, 2, 64, "mma"), (2, 130, 4, 2, 128, "mma"), (1, 257, 8, 8, 128, "mma"),
-    (2, 128, 4, 2, 128, "tc"), (2, 130, 4, 2, 128, "tc"), (1, 257, 8, 8, 128, "tc"), (2, 192, 14, 2, 64, "tc"),
-    (1, 321, 4, 4, 64, "tc"), (2, 512, 28, 4, 128, "tc"), (1, 1024, 32, 8, 128, "tc")])
-def test_attn_bwd(nat, B, S, n_h, n_kv, d, impl, monkeypatch):
-    """dQ, dK, dV vs fp32 autograd: the mma.sync kernels (short sequences, TL_ATTN_BWD=mma) and the tcgen05 kernels (from one
-    128-row tile upwards; sequence lengths off the 64 / 128 tile grid, GQA groups 1..7, both head sizes)."""
+@pytest.mark.parametrize("impl", ["mma", "wgmma"])
+@pytest.mark.parametrize("B,S,n_h,n_kv,d", [
+    (2, 64, 4, 2, 64), (1, 100, 14, 2, 64), (2, 130, 4, 2, 128), (1, 257, 8, 8, 128), (2, 128, 4, 2, 128), (2, 192, 14, 2, 64),
+    (1, 321, 4, 4, 64), (2, 512, 28, 4, 128), (1, 1024, 32, 8, 128), (2, 384, 12, 2, 128), (1, 200, 6, 3, 64), (1, 40, 4, 2, 128)])
+def test_attn_bwd(nat, monkeypatch, B, S, n_h, n_kv, d, impl):
+    """dQ, dK, dV vs fp32 autograd through both backward forms, each forced for every case: the mma.sync kernels
+    (attention_bwd.cu) and the wgmma kernels (attention_wgmma.cu); sequence lengths on and off the 64-row tile grid, GQA
+    groups 1..7, both head sizes."""
     monkeypatch.setenv("TL_ATTN_BWD", impl)
     q, k, v = rnd(B, S, n_h, d, seed=12, std=0.7), rnd(B, n_kv, S, d, seed=13, std=0.7), rnd(B, n_kv, S, d, seed=14)
     do = rnd(B, S, n_h * d, seed=15)

@@ -147,7 +147,7 @@ def test_generate_bounds_are_checked():
 
 def test_forward_and_backward_packets_through_the_torchnode_adapter():
     """The reference's FORWARD / BACKWARD packets (p2p/torch_node.py:825-836, :865-869) in, reply packets out, over a real
-    stage: what a reference user process would exchange with a B200 worker (SURVEY.md §8 f-4)."""
+    stage: what a reference user process would exchange with an H100 worker (SURVEY.md §8 f-4)."""
     import pickle
     from oracle import wire_oracle as W
     from tensorlink_b200.ml.worker import DistributedWorker

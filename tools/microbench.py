@@ -1,4 +1,4 @@
-"""Kernel micro-benchmarks on one B200 (CUDA events, rotating buffers larger than L2).  Not a bench line."""
+"""Kernel micro-benchmarks on one H100 (CUDA events, rotating buffers larger than L2).  Not a bench line."""
 import json
 import sys
 import os

@@ -6,7 +6,8 @@ holds final norm + lm_head = HEAD layer-equivalents per GEMM):
   dgrad chain     B_k = L_k * b      (+ head dgrad when split)
   weight grads    W_k = n_mb * L_k * w (+ head) once, after the stage's last dgrad
 Stages process micro-batches in order, a stage starts a micro-batch when the neighbour has delivered it.
-Used for DESIGN.md §4.4 / §5 (the model reproduces the measured N = 2 / 4 / 8 step times within 2 %).
+Its unit costs are fixed inputs (tests/test_generate_host_cpu.py pins the step times they give); they have not been
+re-measured on H100.
 
   python tools/pipeline_model.py --stages 8 --layers 28 --mb 16
 """

@@ -15,7 +15,7 @@ ap.add_argument("--model", default="Qwen/Qwen2.5-7B")
 ap.add_argument("--prompt", type=int, default=32)
 ap.add_argument("--new", type=int, default=4)
 ap.add_argument("--graph", action="store_true")
-ap.add_argument("--rows", type=int, default=1, help="rows per decode step (32 = BASELINE config 5: tcgen05 GEMM + split-K path)")
+ap.add_argument("--rows", type=int, default=1, help="rows per decode step (32 = BASELINE config 5: wgmma GEMM + split-K path)")
 ap.add_argument("--max-seq", type=int, default=0, help="KV cache length (> 2048 selects the split-KV decode attention)")
 a = ap.parse_args()
 cfg = get_config(a.model)

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Per-kernel SASS mnemonic counts of libtensorlink_b200.so (cuobjdump -sass): which kernels carry tcgen05 MMAs
-(UTCHMMA), TMEM loads / stores (LDTM / STTM), TMA tensor loads (UTMALDG), bulk copies (UBLKCP, UBLKPF = L2 prefetch),
-legacy mma.sync (HMMA), mbarrier waits (SYNCS), grid-dependency control (ACQBULK / PREEXIT).
+"""Per-kernel SASS mnemonic counts of libtensorlink_b200.so (cuobjdump -sass): which kernels carry wgmma
+(HGMMA), TMA tensor loads (UTMALDG), bulk copies (UBLKCP, UBLKPF = L2 prefetch), mma.sync (HMMA), mbarrier waits
+(SYNCS), grid-dependency control (ACQBULK / PREEXIT).
 
-    python tools/sass_summary.py > profiles/r02_sass_summary.txt
+    python tools/sass_summary.py
 """
 import collections
 import os
@@ -13,7 +13,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "tensorlink_b200", "csrc", "libtensorlink_b200.so")
-KEYS = ["UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UBLKPF", "HMMA", "SYNCS", "ACQBULK", "PREEXIT", "FFMA", "LDS", "LDG", "STG", "ATOM", "RED", "MEMBAR"]
+KEYS = ["HGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "UBLKPF", "HMMA", "SYNCS", "ACQBULK", "PREEXIT", "FFMA", "LDS", "LDG", "STG", "ATOM", "RED", "MEMBAR"]
 
 
 def main():
@@ -33,7 +33,7 @@ def main():
             counts[cur][op] += 1
             counts[cur]["_total"] += 1
     demangled = subprocess.run(["c++filt"], input="\n".join(counts), capture_output=True, text=True).stdout.splitlines()
-    print(f"# SASS mnemonic counts per kernel, {os.path.relpath(LIB, ROOT)} (sm_100a), `python tools/sass_summary.py`")
+    print(f"# SASS mnemonic counts per kernel, {os.path.relpath(LIB, ROOT)} (sm_90a), `python tools/sass_summary.py`")
     print("# columns: " + " ".join(KEYS) + " | total instructions")
     rows = []
     for (mangled, c), name in zip(counts.items(), demangled):
