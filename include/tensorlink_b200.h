@@ -96,7 +96,7 @@ int tl_rope_table(const float* inv_freq, void* cos_tab, void* sin_tab, int max_p
 
 /* ---- K3 + KV-cache append (+ Qwen3 q/k RMSNorm, modeling_qwen3.py:248-264):
  * qkv[n, (n_h+2n_kv)*d] (post-bias) -> q_out[n, n_h*d] rotated; K/V written to
- * cache[b, kv_head, pos, d] with b = n / S, pos = pos0[b or 0] + n % S (pos0 read from device memory so a
+ * cache[b, kv_head, pos, d] with b = n / S, pos = *pos0 + n % S (pos0 read from device memory so a
  * captured CUDA graph can be replayed while the position advances). q_norm_w/k_norm_w may be NULL. */
 int tl_rope_kv_fwd(const void* qkv, void* q_out, void* k_cache, void* v_cache, const int32_t* pos0_dev,
                    const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w,
@@ -120,6 +120,31 @@ int tl_attn_decode_fwd(const void* q, const void* k_cache, const void* v_cache, 
 int tl_attn_decode_fused(const void* qkv, void* k_cache, void* v_cache, void* out, const int32_t* pos_dev,
                          const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w,
                          float eps, int B, int n_h, int n_kv, int d, int T_max, float scale, void* stream);
+
+/* ---- left-padded batches (HF's layout for batched generation): the four entry points above, each with one more
+ * argument, kv_start_dev (device int32[B]).  kv_start[b] is the number of leading pad slots of row b (at most its
+ * cache length - 1, so every row keeps at least one real key):
+ *   - cache slot t of row b holds the token at rotary position t - kv_start[b]; pad slots (t < kv_start[b]) are
+ *     still written, rotated at position 0, and are never attended;
+ *   - attention reads keys kv_start[b]..(last valid key) of row b only: the cache below kv_start may hold anything
+ *     (NaN included) and is not read by the tensor-core kernels, and split-KV partials lying wholly below it are skipped;
+ *   - a query row below kv_start[b] (a pad token of the prompt) gets out = 0 and lse = -inf.
+ * The write position and the KV length stay scalar and shared by all rows, as in the entry points above.  With every
+ * kv_start[b] = 0 each result equals the plain entry point's bit for bit. */
+int tl_rope_kv_fwd_rows(const void* qkv, void* q_out, void* k_cache, void* v_cache, const int32_t* pos0_dev,
+                        const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w,
+                        float eps, int n_tokens, int S, int n_h, int n_kv, int d, int T_max,
+                        const int32_t* kv_start_dev, void* stream);
+int tl_attn_prefill_fwd_rows(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B,
+                             int S, int past_len, int n_h, int n_kv, int d, int T_max, float scale,
+                             const int32_t* kv_start_dev, void* stream);
+int tl_attn_decode_fwd_rows(const void* q, const void* k_cache, const void* v_cache, void* out,
+                            const int32_t* kv_len_dev, void* workspace, size_t ws_bytes, int B, int n_h, int n_kv,
+                            int d, int T_max, float scale, const int32_t* kv_start_dev, void* stream);
+int tl_attn_decode_fused_rows(const void* qkv, void* k_cache, void* v_cache, void* out, const int32_t* pos_dev,
+                              const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w,
+                              float eps, int B, int n_h, int n_kv, int d, int T_max, float scale,
+                              const int32_t* kv_start_dev, void* stream);
 
 /* ---- K7  final norm + lm_head + greedy argmax for M <= 8 rows: ids[m] = argmax_v bf16(norm(x)[m,:]·W[v,:])
  * (lowest index wins ties, as torch.argmax).  logits_out (bf16 [M,V]) optional.

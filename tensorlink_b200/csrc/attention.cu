@@ -35,13 +35,15 @@ __device__ __forceinline__ void mma_bf16_16816(float* c, const uint32_t* a, uint
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-template <int D>
+// ROWS: keys below kv_start[b] (left padding of row b) are never attended: they are zero-filled on load and masked, the
+// KV loop starts at tile kv_start / 64, and a query tile whose every row sits below kv_start writes zeros (lse = -inf).
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(FA_THREADS) attn_prefill_kernel(const bf16* __restrict__ q,
                                                                    const bf16* __restrict__ k_cache,
                                                                    const bf16* __restrict__ v_cache,
                                                                    bf16* __restrict__ out, float* __restrict__ lse,
                                                                    int S, int past_len, int n_h, int n_kv, int T_max,
-                                                                   float scale_log2) {
+                                                                   float scale_log2, const int32_t* __restrict__ kv_start) {
     constexpr int LDS = D + 8;   // padded row (elements): conflict-free ldmatrix
     extern __shared__ __align__(16) unsigned char smem_raw[];
     bf16* sQ = reinterpret_cast<bf16*>(smem_raw);          // [64][LDS]
@@ -60,6 +62,23 @@ __global__ void __launch_bounds__(FA_THREADS) attn_prefill_kernel(const bf16* __
     const bf16* kg = k_cache + ((size_t)b * n_kv + kvh) * T_max * D;
     const bf16* vg = v_cache + ((size_t)b * n_kv + kvh) * T_max * D;
     constexpr int CPR = D / 8;   // 16-byte chunks per row
+    int k_start = 0, t0 = 0;                                   // first valid key and its tile
+    if constexpr (ROWS) {
+        k_start = kv_start[b];
+        if (min(T, past_len + q0 + FA_BQ) <= k_start) {        // every query row of this tile is a pad row
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int row = q0 + warp * 16 + g + r * 8;
+                if (row >= S) continue;
+                bf16* dst = out + ((size_t)b * S + row) * n_h * D + (size_t)h * D;
+#pragma unroll
+                for (int i = 0; i < D / 8; ++i) *reinterpret_cast<uint32_t*>(dst + i * 8 + 2 * t4) = 0u;
+                if (lse && t4 == 0) lse[((size_t)b * n_h + h) * S + row] = -INFINITY;
+            }
+            return;
+        }
+        t0 = k_start / FA_BKV;
+    }
 
     for (int c = tid; c < FA_BQ * CPR; c += FA_THREADS) {
         const int r = c / CPR, cc = c - r * CPR;
@@ -69,7 +88,7 @@ __global__ void __launch_bounds__(FA_THREADS) attn_prefill_kernel(const bf16* __
     auto load_kv = [&](int buf, int kv0) {
         for (int c = tid; c < FA_BKV * CPR; c += FA_THREADS) {
             const int r = c / CPR, cc = c - r * CPR;
-            const bool ok = (kv0 + r) < T;
+            const bool ok = (kv0 + r) < T && (!ROWS || (kv0 + r) >= k_start);   // pad slots load as zeros
             const size_t off = (size_t)(ok ? kv0 + r : 0) * D + cc * 8;
             cp_async16(sK + (buf * FA_BKV + r) * LDS + cc * 8, kg + off, ok);
             cp_async16(sV + (buf * FA_BKV + r) * LDS + cc * 8, vg + off, ok);
@@ -77,7 +96,7 @@ __global__ void __launch_bounds__(FA_THREADS) attn_prefill_kernel(const bf16* __
     };
     const int kv_end = min(T, past_len + q0 + FA_BQ);          // causal upper bound for this query tile
     const int n_tiles = (kv_end + FA_BKV - 1) / FA_BKV;
-    load_kv(0, 0);
+    load_kv(t0 & 1, t0 * FA_BKV);
     cp_async_commit();
 
     float o[D / 8][4];
@@ -87,13 +106,13 @@ __global__ void __launch_bounds__(FA_THREADS) attn_prefill_kernel(const bf16* __
     uint32_t qf[D / 16][4];
     const int qrow_abs0 = past_len + q0 + warp * 16 + g;       // absolute position of row g (row g+8: +8)
 
-    for (int it = 0; it < n_tiles; ++it) {
+    for (int it = t0; it < n_tiles; ++it) {
         const int buf = it & 1;
         if (it + 1 < n_tiles) load_kv(buf ^ 1, (it + 1) * FA_BKV);
         cp_async_commit();
         cp_async_wait<1>();
         __syncthreads();
-        if (it == 0) {
+        if (it == t0) {
 #pragma unroll
             for (int ks = 0; ks < D / 16; ++ks)
                 ldmatrix_x4(qf[ks], sQ + (warp * 16 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8);
@@ -125,6 +144,7 @@ __global__ void __launch_bounds__(FA_THREADS) attn_prefill_kernel(const bf16* __
                 const int qpos = qrow_abs0 + ((e >> 1) ? 8 : 0);
                 float v = s[i][e] * scale_log2;
                 if (key > qpos || key >= T) v = -INFINITY;
+                if constexpr (ROWS) if (key < k_start) v = -INFINITY;
                 s[i][e] = v;
                 mx[e >> 1] = fmaxf(mx[e >> 1], v);
             }
@@ -199,18 +219,24 @@ constexpr int DEC_CHUNK_MMA = 256;      // keys per CTA of the tensor-core split
 // partial record per (b, kv head, split): m[REP], l[REP], o[REP][D]  (fp32)
 __host__ __device__ inline size_t dec_rec_floats(int n_rep, int D) { return (size_t)n_rep * (2 + D); }
 
-template <int D>
+// ROWS: keys below kv_start[b] are never attended; a split wholly below it is not computed (the reduce skips it)
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(const bf16* __restrict__ q,
                                                                         const bf16* __restrict__ k_cache,
                                                                         const bf16* __restrict__ v_cache,
                                                                         float* __restrict__ ws,
                                                                         const int32_t* __restrict__ kv_len_dev,
                                                                         int n_h, int n_kv, int T_max, int n_splits,
-                                                                        float scale_log2) {
+                                                                        float scale_log2, const int32_t* __restrict__ kv_start) {
     const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
     const int kv_len = *kv_len_dev;
     const int c0 = split * DEC_CHUNK;
     if (c0 >= kv_len) return;
+    int k_start = 0;
+    if constexpr (ROWS) {
+        k_start = kv_start[b];
+        if (c0 + DEC_CHUNK <= k_start) return;
+    }
     const int n_rep = n_h / n_kv;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     __shared__ __align__(16) float sq[DEC_MAX_REP][D];
@@ -226,7 +252,7 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(const bf
     __syncthreads();
     // ---- phase A: one key per thread, n_rep dot products
     const int key = c0 + tid;
-    const bool valid = key < kv_len;
+    const bool valid = key < kv_len && (!ROWS || key >= k_start);
     float sc[DEC_MAX_REP];
 #pragma unroll
     for (int r = 0; r < DEC_MAX_REP; ++r) sc[r] = 0.f;
@@ -288,7 +314,8 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(const bf
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[r][j] = 0.f;
     const int nk = min(DEC_CHUNK, kv_len - c0);
-    for (int kk = kgi; kk < nk; kk += KG) {
+    const int k_lo = ROWS ? max(k_start - c0, 0) : 0;           // V rows of pad slots are never read
+    for (int kk = k_lo + kgi; kk < nk; kk += KG) {
         const uint4 vv = *reinterpret_cast<const uint4*>(v_cache + (((size_t)b * n_kv + kvh) * T_max + c0 + kk) * D + dd0);
         const uint32_t* v32 = reinterpret_cast<const uint32_t*>(&vv);
         float vf[8];
@@ -348,11 +375,12 @@ __global__ void __launch_bounds__(DEC_THREADS) attn_decode_split_kernel(const bf
 // shared memory with cp.async (coalesced 16-byte pieces, a ring of two 64-key tiles: the next tile is in flight while one
 // is used; DEC_CHUNK_MMA = 256 keys per CTA), each of the 4 warps owns 16 keys of every 64-key tile with its own online-softmax state, and the 4 states are merged
 // through shared memory into the (m, l, o) record the reduce kernel below expects.
-template <int D>
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(FA_THREADS) attn_decode_mma_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k_cache,
                                                                       const bf16* __restrict__ v_cache, float* __restrict__ ws,
                                                                       const int32_t* __restrict__ kv_len_dev, int n_h, int n_kv,
-                                                                      int T_max, int n_splits, float scale_log2) {
+                                                                      int T_max, int n_splits, float scale_log2,
+                                                                      const int32_t* __restrict__ kv_start) {
     constexpr int LDS = D + 8;
     constexpr int CPR = D / 8;
     constexpr int NT = 2;                                  // shared-memory ring: two 64-key tiles
@@ -360,6 +388,12 @@ __global__ void __launch_bounds__(FA_THREADS) attn_decode_mma_kernel(const bf16*
     const int kv_len = *kv_len_dev;
     const int c0 = split * DEC_CHUNK_MMA;
     if (c0 >= kv_len) return;
+    int k_start = 0, t0 = 0;                               // ROWS: first valid key, first tile of this split holding one
+    if constexpr (ROWS) {
+        k_start = kv_start[b];
+        if (c0 + DEC_CHUNK_MMA <= k_start) return;         // wholly below the start: the reduce skips this split
+        t0 = max(k_start - c0, 0) / FA_BKV;
+    }
     const int n_rep = n_h / n_kv;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     bf16* sQ = reinterpret_cast<bf16*>(smem_raw);          // [16][LDS]
@@ -379,24 +413,24 @@ __global__ void __launch_bounds__(FA_THREADS) attn_decode_mma_kernel(const bf16*
         const int kv0 = c0 + t * FA_BKV, buf = t & 1;
         for (int c = tid; c < FA_BKV * CPR; c += FA_THREADS) {
             const int r = c / CPR, cc = c - r * CPR;
-            const bool ok = (kv0 + r) < kv_len;
+            const bool ok = (kv0 + r) < kv_len && (!ROWS || (kv0 + r) >= k_start);   // pad slots load as zeros
             const size_t off = (size_t)(ok ? kv0 + r : 0) * D + cc * 8;
             cp_async16(sK + (buf * FA_BKV + r) * LDS + cc * 8, kg + off, ok);
             cp_async16(sV + (buf * FA_BKV + r) * LDS + cc * 8, vg + off, ok);
         }
         cp_async_commit();                                  // (the q rows ride in the first group)
     };
-    load_tile(0);
-    if (n_tiles > 1) load_tile(1);
+    load_tile(t0);
+    if (t0 + 1 < n_tiles) load_tile(t0 + 1);
     float o[D / 8][4];
 #pragma unroll
     for (int i = 0; i < D / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
     uint32_t qf[D / 16][4];
-    for (int t = 0; t < n_tiles; ++t) {
+    for (int t = t0; t < n_tiles; ++t) {
         if (t + 1 < n_tiles) cp_async_wait<1>(); else cp_async_wait<0>();     // tile t has landed (t+1 may be in flight)
         __syncthreads();
-        if (t == 0) {
+        if (t == t0) {
 #pragma unroll
             for (int ks = 0; ks < D / 16; ++ks)
                 ldmatrix_x4(qf[ks], sQ + (lane & 15) * LDS + ks * 16 + (lane >> 4) * 8);
@@ -421,7 +455,7 @@ __global__ void __launch_bounds__(FA_THREADS) attn_decode_mma_kernel(const bf16*
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int key = key0 + i * 8 + 2 * t4 + (e & 1);
-                const float v = key < kv_len ? sc[i][e] * scale_log2 : -INFINITY;
+                const float v = (key < kv_len && (!ROWS || key >= k_start)) ? sc[i][e] * scale_log2 : -INFINITY;
                 sc[i][e] = v;
                 mx[e >> 1] = fmaxf(mx[e >> 1], v);
             }
@@ -514,18 +548,21 @@ __global__ void __launch_bounds__(FA_THREADS) attn_decode_mma_kernel(const bf16*
     }
 }
 
-template <int D>
+// ROWS: the splits wholly below kv_start[b] were not computed and are not read
+template <int D, bool ROWS>
 __global__ void attn_decode_reduce_kernel(const float* __restrict__ ws, bf16* __restrict__ out,
-                                          const int32_t* __restrict__ kv_len_dev, int n_h, int n_kv, int n_splits, int chunk) {
+                                          const int32_t* __restrict__ kv_len_dev, int n_h, int n_kv, int n_splits, int chunk,
+                                          const int32_t* __restrict__ kv_start) {
     const int h = blockIdx.x, b = blockIdx.y, dd = threadIdx.x;
     const int n_rep = n_h / n_kv, kvh = h / n_rep, r = h - kvh * n_rep;
     const int kv_len = *kv_len_dev;
     const int ns = min(n_splits, (kv_len + chunk - 1) / chunk);
+    const int s0 = ROWS ? kv_start[b] / chunk : 0;
     const float* base = ws + ((size_t)b * n_kv + kvh) * n_splits * dec_rec_floats(n_rep, D);
     float M = -INFINITY;
-    for (int s = 0; s < ns; ++s) M = fmaxf(M, base[s * dec_rec_floats(n_rep, D) + r]);
+    for (int s = s0; s < ns; ++s) M = fmaxf(M, base[s * dec_rec_floats(n_rep, D) + r]);
     float L = 0.f, O = 0.f;
-    for (int s = 0; s < ns; ++s) {
+    for (int s = s0; s < ns; ++s) {
         const float* rec = base + s * dec_rec_floats(n_rep, D);
         const float w = exp2f(rec[r] - M);
         L += rec[n_rep + r] * w;
@@ -538,41 +575,62 @@ __global__ void attn_decode_reduce_kernel(const float* __restrict__ ws, bf16* __
 
 namespace tl {
 int attn_prefill_wgmma(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B, int S, int past_len,
-                       int n_h, int n_kv, int d, int T_max, float scale, cudaStream_t st);
+                       int n_h, int n_kv, int d, int T_max, float scale, const int32_t* kv_start, cudaStream_t st);
+
+// kv_start (int32[B], device) non-null: the left-padded instantiations (ROWS)
+static int attn_prefill_launch(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B, int S,
+                               int past_len, int n_h, int n_kv, int d, int T_max, float scale, const int32_t* kv_start,
+                               cudaStream_t st, const char* what) {
+    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "%s: head_dim %d not in {64,128}", what, d);
+    TL_REQUIRE(n_kv > 0 && n_h % n_kv == 0, TL_ERR_INVALID, "%s: n_h %% n_kv != 0", what);
+    TL_REQUIRE(past_len >= 0 && past_len + S <= T_max, TL_ERR_INVALID,
+               "%s: past_len %d + S %d exceeds cache T_max %d", what, past_len, S, T_max);
+    if (B == 0 || S == 0) return TL_OK;
+    {   // wgmma kernel (attention_wgmma.cu) from one full 64-row query tile upwards; TL_ATTN_IMPL=mma|wgmma forces a path
+        const char* e = getenv("TL_ATTN_IMPL");          // read per call: tests flip it
+        const int impl = !e ? 0 : (e[0] == 'm' ? 1 : (e[0] == 'w' ? 2 : 0));
+        if (impl == 2 || (impl == 0 && S >= FA_BQ))
+            return attn_prefill_wgmma(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, T_max, scale, kv_start, st);
+    }
+    const dim3 grid((S + FA_BQ - 1) / FA_BQ, n_h, B);
+    const float sl2 = scale * 1.4426950408889634f;
+    const size_t smem = (size_t)(FA_BQ + 4 * FA_BKV) * (d + 8) * sizeof(bf16);
+#define TL_FA_FWD(D_, ROWS_)                                                                                                \
+    do {                                                                                                                    \
+        static bool done = false;                                                                                           \
+        if (!done) { cudaFuncSetAttribute(attn_prefill_kernel<D_, ROWS_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); done = true; } \
+        attn_prefill_kernel<D_, ROWS_><<<grid, FA_THREADS, smem, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, \
+                                                                        (bf16*)out, lse, S, past_len, n_h, n_kv, T_max, sl2, kv_start); \
+    } while (0)
+    if (kv_start) {
+        if (d == 64) TL_FA_FWD(64, true); else TL_FA_FWD(128, true);
+    } else {
+        if (d == 64) TL_FA_FWD(64, false); else TL_FA_FWD(128, false);
+    }
+#undef TL_FA_FWD
+    return check_launch(what);
 }
+
+static int attn_decode_launch(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* kv_len_dev,
+                              void* workspace, size_t ws_bytes, int B, int n_h, int n_kv, int d, int T_max, float scale,
+                              const int32_t* kv_start, cudaStream_t st, const char* what);
+}  // namespace tl
 
 extern "C" {
 
 int tl_attn_prefill_fwd(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B, int S,
                         int past_len, int n_h, int n_kv, int d, int T_max, float scale, void* stream) {
+    return tl::attn_prefill_launch(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, T_max, scale, nullptr,
+                                   (cudaStream_t)stream, "tl_attn_prefill_fwd");
+}
+
+int tl_attn_prefill_fwd_rows(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B, int S,
+                             int past_len, int n_h, int n_kv, int d, int T_max, float scale, const int32_t* kv_start_dev,
+                             void* stream) {
     using namespace tl;
-    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "tl_attn_prefill_fwd: head_dim %d not in {64,128}", d);
-    TL_REQUIRE(n_kv > 0 && n_h % n_kv == 0, TL_ERR_INVALID, "tl_attn_prefill_fwd: n_h %% n_kv != 0");
-    TL_REQUIRE(past_len >= 0 && past_len + S <= T_max, TL_ERR_INVALID,
-               "tl_attn_prefill_fwd: past_len %d + S %d exceeds cache T_max %d", past_len, S, T_max);
-    if (B == 0 || S == 0) return TL_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    {   // wgmma kernel (attention_wgmma.cu) from one full 64-row query tile upwards; TL_ATTN_IMPL=mma|wgmma forces a path
-        const char* e = getenv("TL_ATTN_IMPL");          // read per call: tests flip it
-        const int impl = !e ? 0 : (e[0] == 'm' ? 1 : (e[0] == 'w' ? 2 : 0));
-        if (impl == 2 || (impl == 0 && S >= FA_BQ))
-            return attn_prefill_wgmma(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, T_max, scale, st);
-    }
-    const dim3 grid((S + FA_BQ - 1) / FA_BQ, n_h, B);
-    const float sl2 = scale * 1.4426950408889634f;
-    const size_t smem = (size_t)(FA_BQ + 4 * FA_BKV) * (d + 8) * sizeof(bf16);
-    if (d == 64) {
-        static bool done = false;
-        if (!done) { cudaFuncSetAttribute(attn_prefill_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); done = true; }
-        attn_prefill_kernel<64><<<grid, FA_THREADS, smem, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                                 (bf16*)out, lse, S, past_len, n_h, n_kv, T_max, sl2);
-    } else {
-        static bool done = false;
-        if (!done) { cudaFuncSetAttribute(attn_prefill_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); done = true; }
-        attn_prefill_kernel<128><<<grid, FA_THREADS, smem, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                                  (bf16*)out, lse, S, past_len, n_h, n_kv, T_max, sl2);
-    }
-    return check_launch("tl_attn_prefill_fwd");
+    TL_REQUIRE(kv_start_dev != nullptr, TL_ERR_INVALID, "tl_attn_prefill_fwd_rows: kv_start_dev is null");
+    return attn_prefill_launch(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, T_max, scale, kv_start_dev,
+                               (cudaStream_t)stream, "tl_attn_prefill_fwd_rows");
 }
 
 size_t tl_attn_decode_ws(int B, int n_h, int d, int T_max) {
@@ -583,17 +641,34 @@ size_t tl_attn_decode_ws(int B, int n_h, int d, int T_max) {
 int tl_attn_decode_fwd(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* kv_len_dev,
                        void* workspace, size_t ws_bytes, int B, int n_h, int n_kv, int d, int T_max, float scale,
                        void* stream) {
+    return tl::attn_decode_launch(q, k_cache, v_cache, out, kv_len_dev, workspace, ws_bytes, B, n_h, n_kv, d, T_max, scale,
+                                  nullptr, (cudaStream_t)stream, "tl_attn_decode_fwd");
+}
+
+int tl_attn_decode_fwd_rows(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* kv_len_dev,
+                            void* workspace, size_t ws_bytes, int B, int n_h, int n_kv, int d, int T_max, float scale,
+                            const int32_t* kv_start_dev, void* stream) {
     using namespace tl;
-    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "tl_attn_decode_fwd: head_dim %d not in {64,128}", d);
+    TL_REQUIRE(kv_start_dev != nullptr, TL_ERR_INVALID, "tl_attn_decode_fwd_rows: kv_start_dev is null");
+    return attn_decode_launch(q, k_cache, v_cache, out, kv_len_dev, workspace, ws_bytes, B, n_h, n_kv, d, T_max, scale,
+                              kv_start_dev, (cudaStream_t)stream, "tl_attn_decode_fwd_rows");
+}
+
+}  // extern "C"
+
+namespace tl {
+static int attn_decode_launch(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* kv_len_dev,
+                              void* workspace, size_t ws_bytes, int B, int n_h, int n_kv, int d, int T_max, float scale,
+                              const int32_t* kv_start, cudaStream_t st, const char* what) {
+    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "%s: head_dim %d not in {64,128}", what, d);
     TL_REQUIRE(n_kv > 0 && n_h % n_kv == 0 && n_h / n_kv <= DEC_MAX_REP, TL_ERR_INVALID,
-               "tl_attn_decode_fwd: GQA group %d/%d unsupported (max %d)", n_h, n_kv, DEC_MAX_REP);
-    TL_REQUIRE(kv_len_dev != nullptr, TL_ERR_INVALID, "tl_attn_decode_fwd: kv_len_dev is null");
+               "%s: GQA group %d/%d unsupported (max %d)", what, n_h, n_kv, DEC_MAX_REP);
+    TL_REQUIRE(kv_len_dev != nullptr, TL_ERR_INVALID, "%s: kv_len_dev is null", what);
     TL_REQUIRE(ws_bytes >= tl_attn_decode_ws(B, n_h, d, T_max), TL_ERR_WORKSPACE,
-               "tl_attn_decode_fwd: workspace %zu < %zu", ws_bytes, tl_attn_decode_ws(B, n_h, d, T_max));
+               "%s: workspace %zu < %zu", what, ws_bytes, tl_attn_decode_ws(B, n_h, d, T_max));
     if (B == 0) return TL_OK;
     const int n_splits = (T_max + DEC_CHUNK - 1) / DEC_CHUNK;
     const float sl2 = scale * 1.4426950408889634f;
-    cudaStream_t st = (cudaStream_t)stream;
     const dim3 g1(n_splits, n_kv, B), g2(n_h, B);
     // split phase on tensor cores (attn_decode_mma_kernel) unless TL_DECODE_ATTN=simt asks for the CUDA-core kernel
     const char* impl = getenv("TL_DECODE_ATTN");
@@ -601,34 +676,39 @@ int tl_attn_decode_fwd(const void* q, const void* k_cache, const void* v_cache, 
         const int ns_m = (T_max + DEC_CHUNK_MMA - 1) / DEC_CHUNK_MMA;
         const dim3 gm(ns_m, n_kv, B);
         const size_t smem = (size_t)(16 + 4 * FA_BKV) * (d + 8) * sizeof(bf16);
-        if (d == 64) {
-            static bool done = false;
-            if (!done) { cudaFuncSetAttribute(attn_decode_mma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); done = true; }
-            attn_decode_mma_kernel<64><<<gm, FA_THREADS, smem, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                                    (float*)workspace, kv_len_dev, n_h, n_kv, T_max, ns_m, sl2);
-            attn_decode_reduce_kernel<64><<<g2, 64, 0, st>>>((const float*)workspace, (bf16*)out, kv_len_dev, n_h, n_kv, ns_m, DEC_CHUNK_MMA);
+#define TL_DEC_MMA(D_, ROWS_)                                                                                               \
+        do {                                                                                                                \
+            static bool done = false;                                                                                       \
+            if (!done) { cudaFuncSetAttribute(attn_decode_mma_kernel<D_, ROWS_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); done = true; } \
+            attn_decode_mma_kernel<D_, ROWS_><<<gm, FA_THREADS, smem, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, \
+                                                                             (float*)workspace, kv_len_dev, n_h, n_kv, T_max, ns_m, sl2, kv_start); \
+            attn_decode_reduce_kernel<D_, ROWS_><<<g2, D_, 0, st>>>((const float*)workspace, (bf16*)out, kv_len_dev, n_h, n_kv, ns_m, \
+                                                                     DEC_CHUNK_MMA, kv_start);                             \
+        } while (0)
+        if (kv_start) {
+            if (d == 64) TL_DEC_MMA(64, true); else TL_DEC_MMA(128, true);
         } else {
-            static bool done = false;
-            if (!done) { cudaFuncSetAttribute(attn_decode_mma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); done = true; }
-            attn_decode_mma_kernel<128><<<gm, FA_THREADS, smem, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                                     (float*)workspace, kv_len_dev, n_h, n_kv, T_max, ns_m, sl2);
-            attn_decode_reduce_kernel<128><<<g2, 128, 0, st>>>((const float*)workspace, (bf16*)out, kv_len_dev, n_h, n_kv, ns_m, DEC_CHUNK_MMA);
+            if (d == 64) TL_DEC_MMA(64, false); else TL_DEC_MMA(128, false);
         }
-        return check_launch("tl_attn_decode_fwd");
+#undef TL_DEC_MMA
+        return check_launch(what);
     }
-    if (d == 64) {
-        attn_decode_split_kernel<64><<<g1, DEC_THREADS, 0, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                                  (float*)workspace, kv_len_dev, n_h, n_kv, T_max, n_splits, sl2);
-        attn_decode_reduce_kernel<64><<<g2, 64, 0, st>>>((const float*)workspace, (bf16*)out, kv_len_dev, n_h, n_kv, n_splits, DEC_CHUNK);
+#define TL_DEC_SIMT(D_, ROWS_)                                                                                              \
+    do {                                                                                                                    \
+        attn_decode_split_kernel<D_, ROWS_><<<g1, DEC_THREADS, 0, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, \
+                                                                         (float*)workspace, kv_len_dev, n_h, n_kv, T_max, n_splits, sl2, kv_start); \
+        attn_decode_reduce_kernel<D_, ROWS_><<<g2, D_, 0, st>>>((const float*)workspace, (bf16*)out, kv_len_dev, n_h, n_kv, n_splits, \
+                                                                 DEC_CHUNK, kv_start);                                     \
+    } while (0)
+    if (kv_start) {
+        if (d == 64) TL_DEC_SIMT(64, true); else TL_DEC_SIMT(128, true);
     } else {
-        attn_decode_split_kernel<128><<<g1, DEC_THREADS, 0, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                                   (float*)workspace, kv_len_dev, n_h, n_kv, T_max, n_splits, sl2);
-        attn_decode_reduce_kernel<128><<<g2, 128, 0, st>>>((const float*)workspace, (bf16*)out, kv_len_dev, n_h, n_kv, n_splits, DEC_CHUNK);
+        if (d == 64) TL_DEC_SIMT(64, false); else TL_DEC_SIMT(128, false);
     }
-    return check_launch("tl_attn_decode_fwd");
+#undef TL_DEC_SIMT
+    return check_launch(what);
 }
-
-}  // extern "C"
+}  // namespace tl
 
 // ================================================================================================ fused decode
 // RoPE (+ Qwen3 q/k-norm) + KV-cache append + single-pass attention for ONE new token per batch row, short
@@ -639,12 +719,14 @@ namespace tl {
 
 constexpr int FD_THREADS = 128, FD_MAX_T = 2048;
 
-template <int D>
+// ROWS: row b is left-padded by kv_start[b] slots: the new token is rotated at position pos - kv_start[b] (it is still
+// written to slot pos) and attends to keys kv_start[b]..pos only
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(FD_THREADS) attn_decode_fused_kernel(
     const bf16* __restrict__ qkv, bf16* __restrict__ k_cache, bf16* __restrict__ v_cache, bf16* __restrict__ out,
     const int32_t* __restrict__ pos_dev, const bf16* __restrict__ cos_tab, const bf16* __restrict__ sin_tab,
     const bf16* __restrict__ q_norm_w, const bf16* __restrict__ k_norm_w, float eps, int n_h, int n_kv, int T_max,
-    float scale_log2) {
+    float scale_log2, const int32_t* __restrict__ kv_start) {
     constexpr int HALF = D / 2;
     // programmatic dependent launch: this grid may become resident while the qkv Linear is still running; wait for its
     // output here, and let the o-proj Linear behind us start prefetching its weights right away
@@ -653,6 +735,12 @@ __global__ void __launch_bounds__(FD_THREADS) attn_decode_fused_kernel(
     const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n_rep = n_h / n_kv, kvh = h / n_rep;
     const int pos = *pos_dev;                       // keys 0..pos-1 are cached; the new token is key `pos`
+    int k_start = 0;                                // ROWS: first key this row attends to; the rotary position is
+    if constexpr (ROWS) {                           // pos - k_start (the tables are read from k_start rows earlier)
+        k_start = kv_start[b];
+        cos_tab -= (size_t)k_start * HALF;
+        sin_tab -= (size_t)k_start * HALF;
+    }
     const int heads = n_h + 2 * n_kv;
     __shared__ __align__(16) float sq[D], sk[D], sv[D];
     __shared__ float sscore[FD_MAX_T + 1];
@@ -705,6 +793,7 @@ __global__ void __launch_bounds__(FD_THREADS) attn_decode_fused_kernel(
     const bf16* vb = v_cache + ((size_t)b * n_kv + kvh) * T_max * D;
     float mx = -INFINITY;
     for (int key = tid; key < pos; key += FD_THREADS) {
+        if constexpr (ROWS) if (key < k_start) continue;
         const uint4* kr = reinterpret_cast<const uint4*>(kb + (size_t)key * D);
         float acc = 0.f;
 #pragma unroll 4
@@ -740,6 +829,7 @@ __global__ void __launch_bounds__(FD_THREADS) attn_decode_fused_kernel(
     const float m_all = s_bc[0];
     float lsum = 0.f;
     for (int key = tid; key <= pos; key += FD_THREADS) {
+        if constexpr (ROWS) if (key < k_start) continue;
         const float p = exp2f(sscore[key] - m_all);
         lsum += p;
         sscore[key] = rbf(p);           // P is cast to bf16 before P·V (SDPA contract); l uses the fp32 value
@@ -755,6 +845,7 @@ __global__ void __launch_bounds__(FD_THREADS) attn_decode_fused_kernel(
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] = 0.f;
     for (int key = kgi; key < pos; key += KG) {
+        if constexpr (ROWS) if (key < k_start) continue;
         const uint4 vv = *reinterpret_cast<const uint4*>(vb + (size_t)key * D + dd0);
         const uint32_t* v32 = reinterpret_cast<const uint32_t*>(&vv);
         const float p = sscore[key];
@@ -791,25 +882,19 @@ __global__ void __launch_bounds__(FD_THREADS) attn_decode_fused_kernel(
 
 }  // namespace tl
 
-extern "C" int tl_attn_decode_fused(const void* qkv, void* k_cache, void* v_cache, void* out, const int32_t* pos_dev,
-                                    const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w,
-                                    float eps, int B, int n_h, int n_kv, int d, int T_max, float scale, void* stream) {
-    using namespace tl;
-    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "tl_attn_decode_fused: head_dim %d not in {64,128}", d);
-    TL_REQUIRE(n_kv > 0 && n_h % n_kv == 0, TL_ERR_INVALID, "tl_attn_decode_fused: n_h %% n_kv != 0");
-    TL_REQUIRE(T_max <= FD_MAX_T, TL_ERR_INVALID, "tl_attn_decode_fused: T_max %d > %d (use the split-KV path)", T_max,
-               FD_MAX_T);
-    TL_REQUIRE(pos_dev != nullptr, TL_ERR_INVALID, "tl_attn_decode_fused: pos_dev is null");
-    if (B == 0) return TL_OK;
-    const float sl2 = scale * 1.4426950408889634f;
-    const dim3 grid(n_h, B);
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(FD_THREADS);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
+namespace tl {
+// launch configuration of the fused decode kernel; programmatic dependent launch is opt-in (see below)
+static int attn_decode_fused_cfg(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, int d, int n_h, int n_kv, int T_max,
+                                 const int32_t* pos_dev, int B, void* stream, const char* what) {
+    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "%s: head_dim %d not in {64,128}", what, d);
+    TL_REQUIRE(n_kv > 0 && n_h % n_kv == 0, TL_ERR_INVALID, "%s: n_h %% n_kv != 0", what);
+    TL_REQUIRE(T_max <= FD_MAX_T, TL_ERR_INVALID, "%s: T_max %d > %d (use the split-KV path)", what, T_max, FD_MAX_T);
+    TL_REQUIRE(pos_dev != nullptr, TL_ERR_INVALID, "%s: pos_dev is null", what);
+    *cfg = {};
+    cfg->gridDim = dim3(n_h, B);
+    cfg->blockDim = dim3(FD_THREADS);
+    cfg->dynamicSmemBytes = 0;
+    cfg->stream = (cudaStream_t)stream;
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     static int use_pdl = -1;
@@ -819,15 +904,50 @@ extern "C" int tl_attn_decode_fused(const void* qkv, void* k_cache, void* v_cach
         // an early-resident attention grid competes with the Linear it overlaps for SMs, so the attribute is opt-in here (TL_PDL_ATTN=1); the weight-streaming Linears keep it on by default
         use_pdl = (!(e && e[0] == '0') && (e2 && e2[0] == '1')) ? 1 : 0;
     }
-    cfg.attrs = attr;
-    cfg.numAttrs = use_pdl ? 1 : 0;
+    cfg->attrs = attr;
+    cfg->numAttrs = use_pdl ? 1 : 0;
+    return TL_OK;
+}
+}  // namespace tl
+
+extern "C" int tl_attn_decode_fused(const void* qkv, void* k_cache, void* v_cache, void* out, const int32_t* pos_dev,
+                                    const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w,
+                                    float eps, int B, int n_h, int n_kv, int d, int T_max, float scale, void* stream) {
+    using namespace tl;
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[1];
+    const int rc = attn_decode_fused_cfg(&cfg, attr, d, n_h, n_kv, T_max, pos_dev, B, stream, "tl_attn_decode_fused");
+    if (rc != TL_OK || B == 0) return rc;
+    const float sl2 = scale * 1.4426950408889634f;
     if (d == 64)
-        cudaLaunchKernelEx(&cfg, attn_decode_fused_kernel<64>, (const bf16*)qkv, (bf16*)k_cache, (bf16*)v_cache, (bf16*)out, pos_dev,
-                           (const bf16*)cos_tab, (const bf16*)sin_tab, (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps, n_h, n_kv,
-                           T_max, sl2);
+        cudaLaunchKernelEx(&cfg, attn_decode_fused_kernel<64, false>, (const bf16*)qkv, (bf16*)k_cache, (bf16*)v_cache, (bf16*)out,
+                           pos_dev, (const bf16*)cos_tab, (const bf16*)sin_tab, (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps,
+                           n_h, n_kv, T_max, sl2, (const int32_t*)nullptr);
     else
-        cudaLaunchKernelEx(&cfg, attn_decode_fused_kernel<128>, (const bf16*)qkv, (bf16*)k_cache, (bf16*)v_cache, (bf16*)out, pos_dev,
-                           (const bf16*)cos_tab, (const bf16*)sin_tab, (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps, n_h, n_kv,
-                           T_max, sl2);
+        cudaLaunchKernelEx(&cfg, attn_decode_fused_kernel<128, false>, (const bf16*)qkv, (bf16*)k_cache, (bf16*)v_cache, (bf16*)out,
+                           pos_dev, (const bf16*)cos_tab, (const bf16*)sin_tab, (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps,
+                           n_h, n_kv, T_max, sl2, (const int32_t*)nullptr);
     return check_launch("tl_attn_decode_fused");
+}
+
+extern "C" int tl_attn_decode_fused_rows(const void* qkv, void* k_cache, void* v_cache, void* out, const int32_t* pos_dev,
+                                         const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w,
+                                         float eps, int B, int n_h, int n_kv, int d, int T_max, float scale,
+                                         const int32_t* kv_start_dev, void* stream) {
+    using namespace tl;
+    TL_REQUIRE(kv_start_dev != nullptr, TL_ERR_INVALID, "tl_attn_decode_fused_rows: kv_start_dev is null");
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[1];
+    const int rc = attn_decode_fused_cfg(&cfg, attr, d, n_h, n_kv, T_max, pos_dev, B, stream, "tl_attn_decode_fused_rows");
+    if (rc != TL_OK || B == 0) return rc;
+    const float sl2 = scale * 1.4426950408889634f;
+    if (d == 64)
+        cudaLaunchKernelEx(&cfg, attn_decode_fused_kernel<64, true>, (const bf16*)qkv, (bf16*)k_cache, (bf16*)v_cache, (bf16*)out,
+                           pos_dev, (const bf16*)cos_tab, (const bf16*)sin_tab, (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps,
+                           n_h, n_kv, T_max, sl2, kv_start_dev);
+    else
+        cudaLaunchKernelEx(&cfg, attn_decode_fused_kernel<128, true>, (const bf16*)qkv, (bf16*)k_cache, (bf16*)v_cache, (bf16*)out,
+                           pos_dev, (const bf16*)cos_tab, (const bf16*)sin_tab, (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps,
+                           n_h, n_kv, T_max, sl2, kv_start_dev);
+    return check_launch("tl_attn_decode_fused_rows");
 }

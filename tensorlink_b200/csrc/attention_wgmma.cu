@@ -44,6 +44,15 @@ __device__ __forceinline__ void aw_zero_rows(unsigned char* tile, int valid) {
     }
     fence_proxy_async();
 }
+// zero rows [0, lo) and [hi, 64) of a tile: the first KV tile of a left-padded row (pad slots below lo hold anything)
+template <int D>
+__device__ __forceinline__ void aw_zero_rows_outside(unsigned char* tile, int lo, int hi) {
+    for (int i = threadIdx.x; i < (D / 64) * AW_ROWS * 8; i += AW_THREADS) {
+        const int box = i / (AW_ROWS * 8), rem = i - box * AW_ROWS * 8, row = rem >> 3;
+        if (row < lo || row >= hi) *reinterpret_cast<uint4*>(tile + box * 8192 + row * 128 + (rem & 7) * 16) = make_uint4(0, 0, 0, 0);
+    }
+    fence_proxy_async();
+}
 
 // S (+)= A·B^T over D (both K-major tiles), 64 x 64 fp32 accumulator
 template <int D>
@@ -77,12 +86,15 @@ __device__ __forceinline__ void aw_zero(float (&v)[R]) {
 }
 
 // ================================================================================================ prefill forward
-template <int D>
+// ROWS: keys below kv_start[b] (left padding of row b) are never attended.  The KV loop starts at tile kv_start / 64,
+// and a query tile whose every row sits below kv_start writes zeros (lse = -inf) without loading K/V.
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(AW_THREADS) attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ,
                                                                     const __grid_constant__ CUtensorMap tmKV_k,
                                                                     const __grid_constant__ CUtensorMap tmKV_v,
                                                                     bf16* __restrict__ out, float* __restrict__ lse, int S,
-                                                                    int past_len, int n_h, int n_kv, int T_max, float sl2) {
+                                                                    int past_len, int n_h, int n_kv, int T_max, float sl2,
+                                                                    const int32_t* __restrict__ kv_start) {
     constexpr int TB = AwTile<D>::BYTES;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -94,15 +106,32 @@ __global__ void __launch_bounds__(AW_THREADS) attn_fwd_wgmma_kernel(const __grid
     const int n_keys = min(T, past_len + q0 + AW_ROWS);  // causal limit of this query tile
     const int n_tiles = (n_keys + AW_ROWS - 1) / AW_ROWS;
     const int kv_row = (b * n_kv + kvh) * T_max;
+    int k_start = 0, t0 = 0;                                  // first valid key and its tile
+    if constexpr (ROWS) {
+        k_start = kv_start[b];
+        if (n_keys <= k_start) {                              // every query row of this tile is a pad row
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int row = q0 + aw_row(0) + 8 * r;
+                if (row >= S) continue;
+                bf16* dst = out + ((size_t)b * S + row) * n_h * D + (size_t)h * D;
+#pragma unroll
+                for (int i = 2 * r; i < D / 2; i += 4) *reinterpret_cast<uint32_t*>(dst + aw_col(i)) = 0u;
+                if (lse && (threadIdx.x & 3) == 0) lse[((size_t)b * n_h + h) * S + row] = -INFINITY;
+            }
+            return;
+        }
+        t0 = k_start / AW_ROWS;
+    }
     if (threadIdx.x == 0) {
         for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
         fence_barrier_init();
         mbar_expect_tx(&bars[0], TB);
         aw_load<D>(sQ, &tmQ, &bars[0], b * S + q0, h * D);
-        for (int t = 0; t < 2 && t < n_tiles; ++t) {
+        for (int t = 0; t < 2 && t0 + t < n_tiles; ++t) {
             mbar_expect_tx(&bars[1 + t], 2 * TB);
-            aw_load<D>(sK + t * 2 * TB, &tmKV_k, &bars[1 + t], kv_row + t * AW_ROWS, 0);
-            aw_load<D>(sK + t * 2 * TB + TB, &tmKV_v, &bars[1 + t], kv_row + t * AW_ROWS, 0);
+            aw_load<D>(sK + t * 2 * TB, &tmKV_k, &bars[1 + t], kv_row + (t0 + t) * AW_ROWS, 0);
+            aw_load<D>(sK + t * 2 * TB + TB, &tmKV_v, &bars[1 + t], kv_row + (t0 + t) * AW_ROWS, 0);
         }
     }
     __syncthreads();
@@ -111,13 +140,18 @@ __global__ void __launch_bounds__(AW_THREADS) attn_fwd_wgmma_kernel(const __grid
     float o[D / 2], m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
     aw_zero(o);
     const int qpos0 = past_len + q0 + aw_row(0);         // rows aw_row(0) and aw_row(0) + 8
-    for (int t = 0; t < n_tiles; ++t) {
-        const int slot = t & 1;
+    for (int t = t0; t < n_tiles; ++t) {
+        const int slot = (t - t0) & 1;
         unsigned char* k = sK + slot * 2 * TB;
         unsigned char* v = k + TB;
-        mbar_wait(&bars[1 + slot], (t >> 1) & 1);
+        mbar_wait(&bars[1 + slot], ((t - t0) >> 1) & 1);
         const int kv0 = t * AW_ROWS;
-        if (kv0 + AW_ROWS > T) {                         // rows past the valid keys may hold anything: P·V must see zeros
+        if constexpr (ROWS) {
+            if (kv0 < k_start || kv0 + AW_ROWS > T) {         // pad slots below k_start and rows past T: P·V must see zeros
+                aw_zero_rows_outside<D>(v, k_start - kv0, T - kv0);
+                __syncthreads();
+            }
+        } else if (kv0 + AW_ROWS > T) {                  // rows past the valid keys may hold anything: P·V must see zeros
             aw_zero_rows<D>(v, T - kv0);
             __syncthreads();
         }
@@ -134,6 +168,7 @@ __global__ void __launch_bounds__(AW_THREADS) attn_fwd_wgmma_kernel(const __grid
             const int key = kv0 + aw_col(i), r = (i >> 1) & 1;
             float x = s[i] * sl2;
             if (key > qpos0 + 8 * r || key >= T) x = -INFINITY;
+            if constexpr (ROWS) if (key < k_start) x = -INFINITY;
             s[i] = x;
             mx[r] = fmaxf(mx[r], x);
         }
@@ -396,8 +431,9 @@ static void aw_smem_attr(const void* kern, int bytes) {
     if (!done) { cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); done = true; }
 }
 
+// kv_start (int32[B], device) non-null: the left-padded instantiation (ROWS)
 int attn_prefill_wgmma(const void* q, const void* k_cache, const void* v_cache, void* out, float* lse, int B, int S, int past_len,
-                       int n_h, int n_kv, int d, int T_max, float scale, cudaStream_t st) {
+                       int n_h, int n_kv, int d, int T_max, float scale, const int32_t* kv_start, cudaStream_t st) {
     CUtensorMap tq, tk, tv;
     int rc = make_tensor_map(&tq, q, (uint64_t)n_h * d, (uint64_t)B * S, (uint64_t)n_h * d, 64, 64);
     if (rc == TL_OK) rc = make_tensor_map(&tk, k_cache, d, (uint64_t)B * n_kv * T_max, d, 64, 64);
@@ -405,15 +441,19 @@ int attn_prefill_wgmma(const void* q, const void* k_cache, const void* v_cache, 
     if (rc != TL_OK) return rc;
     const dim3 grid((S + AW_ROWS - 1) / AW_ROWS, n_h, B);
     const float sl2 = scale * AW_LOG2E;
-    if (d == 64) {
-        const int smem = 5 * AwTile<64>::BYTES + 1024 + 64;
-        aw_smem_attr<64, 0>((const void*)attn_fwd_wgmma_kernel<64>, smem);
-        attn_fwd_wgmma_kernel<64><<<grid, AW_THREADS, smem, st>>>(tq, tk, tv, (bf16*)out, lse, S, past_len, n_h, n_kv, T_max, sl2);
+#define TL_AW_FWD(D_, ROWS_, WHICH_)                                                                                        \
+    do {                                                                                                                    \
+        const int smem = 5 * AwTile<D_>::BYTES + 1024 + 64;                                                                 \
+        aw_smem_attr<D_, WHICH_>((const void*)attn_fwd_wgmma_kernel<D_, ROWS_>, smem);                                      \
+        attn_fwd_wgmma_kernel<D_, ROWS_><<<grid, AW_THREADS, smem, st>>>(tq, tk, tv, (bf16*)out, lse, S, past_len, n_h, n_kv, \
+                                                                         T_max, sl2, kv_start);                             \
+    } while (0)
+    if (kv_start) {
+        if (d == 64) TL_AW_FWD(64, true, 3); else TL_AW_FWD(128, true, 3);
     } else {
-        const int smem = 5 * AwTile<128>::BYTES + 1024 + 64;
-        aw_smem_attr<128, 0>((const void*)attn_fwd_wgmma_kernel<128>, smem);
-        attn_fwd_wgmma_kernel<128><<<grid, AW_THREADS, smem, st>>>(tq, tk, tv, (bf16*)out, lse, S, past_len, n_h, n_kv, T_max, sl2);
+        if (d == 64) TL_AW_FWD(64, false, 0); else TL_AW_FWD(128, false, 0);
     }
+#undef TL_AW_FWD
     return check_launch("tl_attn_prefill_fwd (wgmma)");
 }
 

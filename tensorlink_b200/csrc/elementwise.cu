@@ -86,7 +86,9 @@ __global__ void rope_table_kernel(const float* __restrict__ inv_freq, bf16* __re
 
 // ------------------------------------------------------------------------------------------------ RoPE + KV append
 // one warp per (token, head) vector; lanes own pairs (i, i + d/2)
-template <int D>
+// ROWS: row b's token at cache slot t sits at rotary position t - kv_start[b] (left-padded rows); the pad slots below
+// kv_start get a negative position and are rotated at position 0 instead (finite, never attended)
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(128) rope_kv_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ q_out,
                                                            bf16* __restrict__ k_cache, bf16* __restrict__ v_cache,
                                                            const int32_t* __restrict__ pos0_dev,
@@ -94,7 +96,8 @@ __global__ void __launch_bounds__(128) rope_kv_fwd_kernel(const bf16* __restrict
                                                            const bf16* __restrict__ sin_tab,
                                                            const bf16* __restrict__ q_norm_w,
                                                            const bf16* __restrict__ k_norm_w, float eps, int n_tokens,
-                                                           int S, int n_h, int n_kv, int T_max) {
+                                                           int S, int n_h, int n_kv, int T_max,
+                                                           const int32_t* __restrict__ kv_start) {
     constexpr int HALF = D / 2;
     constexpr int PAIRS = HALF / 32;   // pairs per lane: 1 (d=64) or 2 (d=128)
     const int heads = n_h + 2 * n_kv;
@@ -104,6 +107,8 @@ __global__ void __launch_bounds__(128) rope_kv_fwd_kernel(const bf16* __restrict
     const int n = gw / heads, h = gw - n * heads;
     const int b = n / S;
     const int pos = (pos0_dev ? *pos0_dev : 0) + (n - b * S);
+    int rpos = pos;                                          // rotary position (the cache slot is always `pos`)
+    if constexpr (ROWS) rpos = max(pos - kv_start[b], 0);
     const bf16* src = qkv + (size_t)n * heads * D + (size_t)h * D;
     float x1[PAIRS], x2[PAIRS];
 #pragma unroll
@@ -139,8 +144,8 @@ __global__ void __launch_bounds__(128) rope_kv_fwd_kernel(const bf16* __restrict
 #pragma unroll
     for (int p = 0; p < PAIRS; ++p) {
         const int i = lane + 32 * p;
-        const float c = bf2f(cos_tab[(size_t)pos * HALF + i]);
-        const float s = bf2f(sin_tab[(size_t)pos * HALF + i]);
+        const float c = bf2f(cos_tab[(size_t)rpos * HALF + i]);
+        const float s = bf2f(sin_tab[(size_t)rpos * HALF + i]);
         // (q * cos) + (rotate_half(q) * sin), every product and the sum rounded to bf16 like torch
         dst[i] = f2bf(rbf(x1[p] * c) + rbf(-x2[p] * s));
         dst[i + HALF] = f2bf(rbf(x2[p] * c) + rbf(x1[p] * s));
@@ -180,28 +185,46 @@ int tl_rope_table(const float* inv_freq, void* cos_tab, void* sin_tab, int max_p
     return check_launch("tl_rope_table");
 }
 
-int tl_rope_kv_fwd(const void* qkv, void* q_out, void* k_cache, void* v_cache, const int32_t* pos0_dev,
-                   const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w, float eps,
-                   int n_tokens, int S, int n_h, int n_kv, int d, int T_max, void* stream) {
+static int rope_kv_launch(const void* qkv, void* q_out, void* k_cache, void* v_cache, const int32_t* pos0_dev,
+                          const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w, float eps,
+                          int n_tokens, int S, int n_h, int n_kv, int d, int T_max, const int32_t* kv_start, void* stream,
+                          const char* what) {
     using namespace tl;
-    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "tl_rope_kv_fwd: head_dim %d not in {64,128}", d);
-    TL_REQUIRE(S > 0 && n_tokens % S == 0, TL_ERR_INVALID, "tl_rope_kv_fwd: n_tokens %d not a multiple of S %d",
-               n_tokens, S);
+    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "%s: head_dim %d not in {64,128}", what, d);
+    TL_REQUIRE(S > 0 && n_tokens % S == 0, TL_ERR_INVALID, "%s: n_tokens %d not a multiple of S %d", what, n_tokens, S);
     if (n_tokens == 0) return TL_OK;
     const long long warps = (long long)n_tokens * (n_h + 2 * n_kv);
     const int grid = (int)((warps + 3) / 4);
     cudaStream_t st = (cudaStream_t)stream;
-    if (d == 64)
-        rope_kv_fwd_kernel<64><<<grid, 128, 0, st>>>((const bf16*)qkv, (bf16*)q_out, (bf16*)k_cache, (bf16*)v_cache,
-                                                     pos0_dev, (const bf16*)cos_tab, (const bf16*)sin_tab,
-                                                     (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps, n_tokens, S,
-                                                     n_h, n_kv, T_max);
-    else
-        rope_kv_fwd_kernel<128><<<grid, 128, 0, st>>>((const bf16*)qkv, (bf16*)q_out, (bf16*)k_cache, (bf16*)v_cache,
-                                                      pos0_dev, (const bf16*)cos_tab, (const bf16*)sin_tab,
-                                                      (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps, n_tokens, S,
-                                                      n_h, n_kv, T_max);
-    return check_launch("tl_rope_kv_fwd");
+#define TL_ROPE_LAUNCH(D_, ROWS_)                                                                                          \
+    rope_kv_fwd_kernel<D_, ROWS_><<<grid, 128, 0, st>>>((const bf16*)qkv, (bf16*)q_out, (bf16*)k_cache, (bf16*)v_cache,   \
+                                                        pos0_dev, (const bf16*)cos_tab, (const bf16*)sin_tab,              \
+                                                        (const bf16*)q_norm_w, (const bf16*)k_norm_w, eps, n_tokens, S,   \
+                                                        n_h, n_kv, T_max, kv_start)
+    if (kv_start) {
+        if (d == 64) TL_ROPE_LAUNCH(64, true); else TL_ROPE_LAUNCH(128, true);
+    } else {
+        if (d == 64) TL_ROPE_LAUNCH(64, false); else TL_ROPE_LAUNCH(128, false);
+    }
+#undef TL_ROPE_LAUNCH
+    return check_launch(what);
+}
+
+int tl_rope_kv_fwd(const void* qkv, void* q_out, void* k_cache, void* v_cache, const int32_t* pos0_dev,
+                   const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w, float eps,
+                   int n_tokens, int S, int n_h, int n_kv, int d, int T_max, void* stream) {
+    return rope_kv_launch(qkv, q_out, k_cache, v_cache, pos0_dev, cos_tab, sin_tab, q_norm_w, k_norm_w, eps, n_tokens, S,
+                          n_h, n_kv, d, T_max, nullptr, stream, "tl_rope_kv_fwd");
+}
+
+int tl_rope_kv_fwd_rows(const void* qkv, void* q_out, void* k_cache, void* v_cache, const int32_t* pos0_dev,
+                        const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w, float eps,
+                        int n_tokens, int S, int n_h, int n_kv, int d, int T_max, const int32_t* kv_start_dev,
+                        void* stream) {
+    using namespace tl;
+    TL_REQUIRE(kv_start_dev != nullptr, TL_ERR_INVALID, "tl_rope_kv_fwd_rows: kv_start_dev is null");
+    return rope_kv_launch(qkv, q_out, k_cache, v_cache, pos0_dev, cos_tab, sin_tab, q_norm_w, k_norm_w, eps, n_tokens, S,
+                          n_h, n_kv, d, T_max, kv_start_dev, stream, "tl_rope_kv_fwd_rows");
 }
 
 }  // extern "C"

@@ -99,6 +99,17 @@ def _left_pad_groups(mask: torch.Tensor):
     return groups
 
 
+def _left_pad_starts(mask: torch.Tensor):
+    """A left-padded batch as (trim, starts): ``trim`` leading columns are pad in every row and are dropped, and row b of
+    the remaining ``S - trim`` columns starts with ``starts[b]`` pad slots.  None when no row is padded; right padding /
+    holes raise (``_left_pad_groups``)."""
+    if _left_pad_groups(mask) is None:
+        return None
+    lengths = (mask != 0).sum(1).cpu()
+    width = int(lengths.max())
+    return mask.shape[1] - width, [width - int(L) for L in lengths.tolist()]
+
+
 EOS_CHECK_EVERY = 16       # decode steps between two host-side "has every row emitted EOS?" checks
 
 
@@ -380,10 +391,10 @@ class DistributedModel(torch.nn.Module):
         return apply_eos(result, S, *self._eos)
 
     def _generate_left_padded(self, input_ids, groups, shape, max_new, streamer, use_graph, sampling):
-        """HF semantics for a left-padded batch: every row attends to its own tokens only, at positions 0..L-1.  Rows of
-        equal real length are generated together (one uniform run per length: the KV cache and RoPE positions of a run
-        start at the row's first real token, so no pad key exists to be masked); the result keeps HF's layout
-        [pads | prompt | new tokens | pad_token_id...]."""
+        """HF semantics for a left-padded batch on a stage without per-row key starts (``supports_kv_start``): every row
+        attends to its own tokens only, at positions 0..L-1.  Rows of equal real length are generated together (one
+        uniform run per length: the KV cache and RoPE positions of a run start at the row's first real token, so no pad
+        key exists to be masked); the result keeps HF's layout [pads | prompt | new tokens | pad_token_id...]."""
         if streamer is not None:
             raise NotImplementedError("streamer with a padded batch (rows finish in separate runs)")
         eos, pad = self._eos
@@ -420,7 +431,12 @@ class DistributedModel(torch.nn.Module):
         default ``torch.initial_seed()``): the same seed reproduces the same tokens (csrc/sample.cu).
         ``input_ids`` [B,S] int64 on the first stage; returns [B,S+new] on every rank.
         ``streamer``: object with ``put(tensor)`` / ``end()`` (HF BaseStreamer protocol), called on rank 0
-        with each new token column, all batch rows (the reference streams row 0 only, worker.py:134-139)."""
+        with each new token column, all batch rows (the reference streams row 0 only, worker.py:134-139).
+        ``attention_mask``: a left-padded batch (HF's layout for batched generation) runs as ONE batch: columns that are
+        pad in every row are dropped, and each row's pad slots are masked out of attention with its RoPE positions
+        starting at its first real token.  The result keeps HF's layout [pads | prompt | new tokens | pad_token_id...].
+        With ``do_sample`` a padded batch draws one stream per micro-batch slot, exactly as an unpadded batch does, so
+        a row's tokens depend on the seed and its place in the batch, not on its prompt length."""
         input_ids = kwargs.pop("input_ids", args[0] if args else None)
         max_new = int(kwargs.pop("max_new_tokens", 20))
         streamer = kwargs.pop("streamer", None)
@@ -438,16 +454,33 @@ class DistributedModel(torch.nn.Module):
         mask = kwargs.pop("attention_mask", None)
         _check_unconsumed(kwargs, "DistributedModel.generate")
         link, st, cfg = self.link, self.stage, self.cfg
-        groups = None
+        groups, padded = None, None
         if link.first and mask is not None:
             if tuple(mask.shape) != tuple(input_ids.shape):
                 raise ValueError(f"attention_mask shape {tuple(mask.shape)} != input_ids shape {tuple(input_ids.shape)}")
-            g = _left_pad_groups(mask)
-            groups = None if g is None else (g, tuple(input_ids.shape))
+            if getattr(st, "supports_kv_start", False):
+                p = _left_pad_starts(mask)
+                # (pad columns common to every row, per-row key starts); the dropped columns return in the result
+                padded = None if p is None else (input_ids[:, :p[0]].cpu(), p[1])
+                if padded is not None:
+                    input_ids = input_ids[:, p[0]:]
+            else:
+                g = _left_pad_groups(mask)
+                groups = None if g is None else (g, tuple(input_ids.shape))
         if self.world > 1:
-            groups = link.broadcast_object(groups)
+            groups, padded = link.broadcast_object((groups, padded))
         if groups is not None:
             return self._generate_left_padded(input_ids, groups[0], groups[1], max_new, streamer, use_graph, sampling)
+        result = self._generate_batch(input_ids, max_new, streamer, use_graph, profile, sampling,
+                                      None if padded is None else padded[1])
+        if padded is not None and padded[0].shape[1]:
+            result = torch.cat([padded[0].to(result.device), result], dim=1)
+        return result
+
+    def _generate_batch(self, input_ids, max_new, streamer, use_graph, profile, sampling, kv_start):
+        """One run of the batch: prefill every micro-batch, then the decode loop.  ``kv_start``: the per-row key starts
+        of a left-padded batch, or None."""
+        link, st, cfg = self.link, self.stage, self.cfg
         shape, sampling = link.broadcast_object((tuple(input_ids.shape), sampling) if link.first else None)
         B, S = shape
         if hasattr(st, "set_sampling"):
@@ -484,7 +517,10 @@ class DistributedModel(torch.nn.Module):
             else:
                 x = torch.empty(b, S, cfg.hidden, dtype=torch.bfloat16, device=dev)
                 link.recv_prev(x)
-            x = st.prefill(x, 0, m)
+            if kv_start is None:
+                x = st.prefill(x, 0, m)
+            else:
+                x = st.prefill(x, 0, m, kv_start=kv_start[m * b:(m + 1) * b])
             if not link.last:
                 link.send_next(x.clone())
             elif ring is not None:                         # first token straight into the first stage's mailbox

@@ -216,6 +216,10 @@ class CudaLayerGroup:
                                          params.v.get(f"l{self.layer_ids[0]}.wqkv") if len(self.layer_ids) else None)
         self.pos_dev = torch.zeros(1, dtype=torch.int32, device=dev)      # next write position in the cache
         self.kvlen_dev = torch.zeros(1, dtype=torch.int32, device=dev)    # valid keys for the decode kernel
+        # left-padded rows: kv_start[b] leading cache slots of row b are pad (never attended; RoPE position = slot -
+        # kv_start[b]).  Set by prefill(kv_start=...), constant through the decode steps that follow it.
+        self.kv_start_dev = torch.zeros(max_batch, dtype=torch.int32, device=dev)
+        self.ragged = False
         self.n_max = max_tokens or max_batch * max_seq
         self._alloc_bufs(min(self.n_max, 8))
         self.dbufs = self._make_bufs(max_batch)       # decode-time buffers: fixed addresses (captured graphs, job lists)
@@ -259,15 +263,20 @@ class CudaLayerGroup:
         self.kvlen_dev.fill_(past_len)
 
     # ------------------------------------------------------------------------------------------ layer bodies
+    def _kv_start(self):
+        """The per-row key starts for the attention and RoPE launches, or None (every row starts at slot 0)."""
+        return self.kv_start_dev if self.ragged else None
+
     def _layer_prefill(self, j: int, x: torch.Tensor, B: int, S: int, past_len: int, w: ShardBuffers):
         """site-packages/transformers/models/qwen2/modeling_qwen2.py:280-310 for N = B*S tokens (GEMM path)."""
         cfg, v, li = self.cfg, self.p.v, self.layer_ids[j]
+        ks = self._kv_start()
         nat.rmsnorm_fwd(x, v[f"l{li}.ln1"], cfg.rms_eps, out=w.h)
         nat.gemm(w.h, v[f"l{li}.wqkv"], out=w.qkv, bias=v.get(f"l{li}.bqkv"))
         nat.rope_kv_fwd(w.qkv, w.q, self.kc[j], self.vc[j], self.pos_dev, self.cos, self.sin, v.get(f"l{li}.qn"),
-                        v.get(f"l{li}.kn"), cfg.rms_eps, S, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim)
+                        v.get(f"l{li}.kn"), cfg.rms_eps, S, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, kv_start=ks)
         nat.attn_prefill_fwd(w.q, self.kc[j], self.vc[j], w.attn, None, B, S, past_len, cfg.n_heads, cfg.n_kv_heads,
-                             cfg.head_dim, self.scale)
+                             cfg.head_dim, self.scale, kv_start=ks)
         nat.gemm(w.attn, v[f"l{li}.wo"], out=x, residual=x)
         nat.rmsnorm_fwd(x, v[f"l{li}.ln2"], cfg.rms_eps, out=w.h)
         nat.gemm(w.h, v[f"l{li}.wgu"], out=w.act, flags=nat.EPI_SWIGLU)
@@ -279,15 +288,16 @@ class CudaLayerGroup:
         """w.qkv (post-bias) -> w.attn for one new token per row.  Short caches: one fused launch (RoPE + append +
         attention); long caches: RoPE/append, split-KV partials, reduce (three launches, parallel over the KV length)."""
         cfg, v = self.cfg, self.p.v
+        ks = self._kv_start()
         if self.T_max <= self.FUSED_DECODE_MAX_T and (cfg.n_heads // cfg.n_kv_heads) <= 8:
             nat.attn_decode_fused(w.qkv, self.kc[j], self.vc[j], w.attn, self.pos_dev, self.cos, self.sin,
                                   v.get(f"l{li}.qn"), v.get(f"l{li}.kn"), cfg.rms_eps, B, cfg.n_heads, cfg.n_kv_heads,
-                                  cfg.head_dim, self.scale)
+                                  cfg.head_dim, self.scale, kv_start=ks)
             return
         nat.rope_kv_fwd(w.qkv, w.q, self.kc[j], self.vc[j], self.pos_dev, self.cos, self.sin, v.get(f"l{li}.qn"),
-                        v.get(f"l{li}.kn"), cfg.rms_eps, 1, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim)
+                        v.get(f"l{li}.kn"), cfg.rms_eps, 1, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, kv_start=ks)
         nat.attn_decode_fwd(w.q, self.kc[j], self.vc[j], w.attn, self.kvlen_dev, self.dec_ws, B, cfg.n_heads,
-                            cfg.n_kv_heads, cfg.head_dim, self.scale)
+                            cfg.n_kv_heads, cfg.head_dim, self.scale, kv_start=ks)
 
     def _layer_decode(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor] = None):
         """Same layer for B <= 8 single-token rows: weight-streaming GEMVs with the norms fused as prologues."""
@@ -324,11 +334,16 @@ class CudaLayerGroup:
         else:
             nat.gemm(w.act, v[f"l{li}.wd"], out=x if out is None else out, residual=x, ws=ws)
 
-    def prefill(self, hidden: torch.Tensor, past_len: int = 0) -> torch.Tensor:
-        """hidden [B,S,H] -> [B,S,H]; appends S positions to the KV cache starting at ``past_len``."""
+    def prefill(self, hidden: torch.Tensor, past_len: int = 0, kv_start=None) -> torch.Tensor:
+        """hidden [B,S,H] -> [B,S,H]; appends S positions to the KV cache starting at ``past_len``.
+        ``kv_start`` (B ints, or None): a left-padded batch, row b's first ``kv_start[b]`` cache slots being pad.  Those
+        slots are never attended and row b's RoPE positions start at its first real token (HF's left-padded generation:
+        position_ids = cumsum(mask) - 1).  The starts hold for the decode steps after this prefill, until the next one;
+        the pad rows of the output are zero."""
         B, S, H = hidden.shape
         if B > self.B_max or past_len + S > self.T_max:
             raise ValueError(f"shard sized for B<={self.B_max}, T<={self.T_max}; got B={B}, T={past_len + S}")
+        self._set_kv_start(kv_start, B, past_len + S)
         N = B * S
         w = self._bufs(N)
         w.x.copy_(hidden.reshape(N, H))
@@ -338,6 +353,17 @@ class CudaLayerGroup:
         self.pos_dev.fill_(past_len + S)
         self.kvlen_dev.fill_(past_len + S)
         return w.x.view(B, S, H)
+
+    def _set_kv_start(self, kv_start, B: int, T: int):
+        if kv_start is None:
+            self.ragged = False
+            return
+        ks = torch.as_tensor(kv_start, dtype=torch.int32).reshape(-1).cpu()
+        if ks.numel() != B or bool((ks < 0).any()) or bool((ks >= T).any()):
+            raise ValueError(f"kv_start needs {B} values in [0, {T}): every row keeps at least one real token")
+        self.kv_start_dev.zero_()
+        self.kv_start_dev[:B].copy_(ks, non_blocking=False)
+        self.ragged = bool((ks != 0).any())
 
     def decode_step_inplace(self, x: torch.Tensor, out: Optional[torch.Tensor] = None, advance: bool = True):
         """x [B,H] updated in place through this shard's layers; one new token per row at position ``pos_dev``.
@@ -371,7 +397,9 @@ class CudaLayerGroup:
         the default per-kernel sequence pays a programmatic-dependent-launch boundary."""
         import os
         cfg = self.cfg
+        # the chain's ATTN job has no per-row key start: a left-padded slot takes the per-kernel sequence
         return (os.environ.get("TL_DECODE_IMPL", "kernels") == "chain" and self.allow_chain and self.num_layers > 0
+                and not self.ragged
                 and B <= min(4, gemv_max_rows()) and cfg.n_kv_heads * B <= 60 and cfg.n_heads // cfg.n_kv_heads <= 8
                 and cfg.head_dim in (64, 128))
 

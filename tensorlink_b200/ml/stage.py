@@ -26,6 +26,7 @@ class CudaStage:
         self.device = torch.device(device)
         self.has_embed, self.has_head = has_embed, has_head
         self.supports_training, self.trainer = bool(training), None
+        self.supports_kv_start = True       # prefill(kv_start=...): left-padded batches run as one batch
         self.params = ShardParams(cfg, layer_ids, has_embed, has_head, self.device, with_grad=training)
         if state_dict is not None:
             self.params.load_hf_state_dict(state_dict)
@@ -55,8 +56,9 @@ class CudaStage:
         """[B,S] int64 -> [B,S,H]  (host-side ``embed_tokens`` in the reference, module.py:1023-1056)."""
         return nat.embed_fwd(ids.contiguous(), self.params.v["embed"])
 
-    def prefill(self, hidden: torch.Tensor, past_len: int = 0, slot: int = 0) -> torch.Tensor:
-        return self.slots[slot].prefill(hidden, past_len)
+    def prefill(self, hidden: torch.Tensor, past_len: int = 0, slot: int = 0, kv_start=None) -> torch.Tensor:
+        """``kv_start``: per-row leading pad slots of a left-padded batch (CudaLayerGroup.prefill)."""
+        return self.slots[slot].prefill(hidden, past_len, kv_start)
 
     def head_logits(self, hidden: torch.Tensor) -> torch.Tensor:
         """final norm + lm_head over [N,H] -> bf16 logits [N,V]."""
@@ -135,7 +137,8 @@ class CudaStage:
         if not use_graph:
             self._decode_body(slot, B, ring)
             return
-        key = (slot, B) if ring is None else (slot, B, id(ring))
+        ragged = self.slots[slot].ragged          # the captured launches differ (the _rows kernels, no decode chain)
+        key = (slot, B, ragged) if ring is None else (slot, B, ragged, id(ring))
         g = self.graphs.get(key)
         if g is None:
             # warm up outside capture (first-use attribute setting, tensor-map cache), restoring the state it touches

@@ -48,6 +48,14 @@ _SIGS = {
     "tl_attn_decode_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int,
                                    c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "tl_attn_decode_fused": (c_int, [c_void_p] * 9 + [c_float, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+    "tl_rope_kv_fwd_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "tl_attn_prefill_fwd_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                         c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "tl_attn_decode_fwd_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int,
+                                        c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "tl_attn_decode_fused_rows": (c_int, [c_void_p] * 9 + [c_float, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
+                                                           c_void_p]),
     "tl_decode_chain_ws": (c_size_t, [c_int, c_int, c_int, c_int]),
     "tl_decode_chain_trace": (c_int, [c_void_p, c_int]),
     "tl_decode_chain": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),
@@ -283,35 +291,60 @@ def rope_table(inv_freq: torch.Tensor, max_pos: int):
     return cos, sin
 
 
-def rope_kv_fwd(qkv, q_out, k_cache, v_cache, pos0_dev, cos_tab, sin_tab, q_norm_w, k_norm_w, eps, S, n_h, n_kv, d):
+def _kv_start(kv_start, B):
+    """``kv_start``: int32[>= B] on the device, row b's leading pad slots (include/tensorlink_b200.h, left-padded batches)"""
+    if kv_start.dtype != torch.int32 or not kv_start.is_cuda or kv_start.numel() < B or not kv_start.is_contiguous():
+        raise NativeError(f"kv_start must be a contiguous int32 CUDA tensor of at least {B} rows")
+
+
+def rope_kv_fwd(qkv, q_out, k_cache, v_cache, pos0_dev, cos_tab, sin_tab, q_norm_w, k_norm_w, eps, S, n_h, n_kv, d,
+                kv_start=None):
+    """``kv_start`` (int32[B] device, optional): left-padded rows, through ``tl_rope_kv_fwd_rows``."""
     require_device()
     _bf16(qkv, q_out, k_cache, v_cache, cos_tab, sin_tab, q_norm_w, k_norm_w)
     n_tokens = qkv.shape[0]
     T_max = k_cache.shape[2]
-    _check(load().tl_rope_kv_fwd(_p(qkv), _p(q_out), _p(k_cache), _p(v_cache), _p(pos0_dev), _p(cos_tab), _p(sin_tab),
-                                 _p(q_norm_w), _p(k_norm_w), eps, n_tokens, S, n_h, n_kv, d, T_max, _stream()),
-           "tl_rope_kv_fwd")
+    if kv_start is None:
+        _check(load().tl_rope_kv_fwd(_p(qkv), _p(q_out), _p(k_cache), _p(v_cache), _p(pos0_dev), _p(cos_tab), _p(sin_tab),
+                                     _p(q_norm_w), _p(k_norm_w), eps, n_tokens, S, n_h, n_kv, d, T_max, _stream()),
+               "tl_rope_kv_fwd")
+        return
+    _kv_start(kv_start, n_tokens // S)
+    _check(load().tl_rope_kv_fwd_rows(_p(qkv), _p(q_out), _p(k_cache), _p(v_cache), _p(pos0_dev), _p(cos_tab), _p(sin_tab),
+                                      _p(q_norm_w), _p(k_norm_w), eps, n_tokens, S, n_h, n_kv, d, T_max, _p(kv_start),
+                                      _stream()), "tl_rope_kv_fwd_rows")
 
 
-def attn_prefill_fwd(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, scale):
+def attn_prefill_fwd(q, k_cache, v_cache, out, lse, B, S, past_len, n_h, n_kv, d, scale, kv_start=None):
     require_device()
     _bf16(q, k_cache, v_cache, out)
     T_max = k_cache.shape[2]
-    _check(load().tl_attn_prefill_fwd(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(lse), B, S, past_len, n_h, n_kv, d,
-                                      T_max, scale, _stream()), "tl_attn_prefill_fwd")
+    if kv_start is None:
+        _check(load().tl_attn_prefill_fwd(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(lse), B, S, past_len, n_h, n_kv, d,
+                                          T_max, scale, _stream()), "tl_attn_prefill_fwd")
+        return
+    _kv_start(kv_start, B)
+    _check(load().tl_attn_prefill_fwd_rows(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(lse), B, S, past_len, n_h, n_kv, d,
+                                           T_max, scale, _p(kv_start), _stream()), "tl_attn_prefill_fwd_rows")
 
 
 def attn_decode_ws(B, n_h, d, T_max) -> int:
     return int(load().tl_attn_decode_ws(B, n_h, d, T_max))
 
 
-def attn_decode_fwd(q, k_cache, v_cache, out, kv_len_dev, ws, B, n_h, n_kv, d, scale):
+def attn_decode_fwd(q, k_cache, v_cache, out, kv_len_dev, ws, B, n_h, n_kv, d, scale, kv_start=None):
     require_device()
     _bf16(q, k_cache, v_cache, out)
     T_max = k_cache.shape[2]
-    _check(load().tl_attn_decode_fwd(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(kv_len_dev), _p(ws),
-                                     ws.numel() * ws.element_size(), B, n_h, n_kv, d, T_max, scale, _stream()),
-           "tl_attn_decode_fwd")
+    if kv_start is None:
+        _check(load().tl_attn_decode_fwd(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(kv_len_dev), _p(ws),
+                                         ws.numel() * ws.element_size(), B, n_h, n_kv, d, T_max, scale, _stream()),
+               "tl_attn_decode_fwd")
+        return
+    _kv_start(kv_start, B)
+    _check(load().tl_attn_decode_fwd_rows(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(kv_len_dev), _p(ws),
+                                          ws.numel() * ws.element_size(), B, n_h, n_kv, d, T_max, scale, _p(kv_start),
+                                          _stream()), "tl_attn_decode_fwd_rows")
 
 
 def lmhead_ws(M, V) -> int:
@@ -503,11 +536,18 @@ def adamw_step(param, grad, m, v, lr, beta1, beta2, eps, wd, step: int, decouple
                                 int(decoupled), _stream()), "tl_adamw_step")
 
 
-def attn_decode_fused(qkv, k_cache, v_cache, out, pos_dev, cos_tab, sin_tab, q_norm_w, k_norm_w, eps, B, n_h, n_kv, d, scale):
+def attn_decode_fused(qkv, k_cache, v_cache, out, pos_dev, cos_tab, sin_tab, q_norm_w, k_norm_w, eps, B, n_h, n_kv, d, scale,
+                      kv_start=None):
     require_device(); _bf16(qkv, k_cache, v_cache, out)
-    _check(load().tl_attn_decode_fused(_p(qkv), _p(k_cache), _p(v_cache), _p(out), _p(pos_dev), _p(cos_tab), _p(sin_tab),
-                                       _p(q_norm_w), _p(k_norm_w), eps, B, n_h, n_kv, d, k_cache.shape[2], scale, _stream()),
-           "tl_attn_decode_fused")
+    if kv_start is None:
+        _check(load().tl_attn_decode_fused(_p(qkv), _p(k_cache), _p(v_cache), _p(out), _p(pos_dev), _p(cos_tab), _p(sin_tab),
+                                           _p(q_norm_w), _p(k_norm_w), eps, B, n_h, n_kv, d, k_cache.shape[2], scale, _stream()),
+               "tl_attn_decode_fused")
+        return
+    _kv_start(kv_start, B)
+    _check(load().tl_attn_decode_fused_rows(_p(qkv), _p(k_cache), _p(v_cache), _p(out), _p(pos_dev), _p(cos_tab), _p(sin_tab),
+                                            _p(q_norm_w), _p(k_norm_w), eps, B, n_h, n_kv, d, k_cache.shape[2], scale,
+                                            _p(kv_start), _stream()), "tl_attn_decode_fused_rows")
 
 
 def decode_chain_ws(M: int, n_h: int, n_kv: int, d: int) -> int:
