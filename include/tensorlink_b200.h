@@ -145,6 +145,16 @@ int tl_attn_decode_fused_rows(const void* qkv, void* k_cache, void* v_cache, voi
                               const void* cos_tab, const void* sin_tab, const void* q_norm_w, const void* k_norm_w,
                               float eps, int B, int n_h, int n_kv, int d, int T_max, float scale,
                               const int32_t* kv_start_dev, void* stream);
+/* The attention backward of a left-padded training batch: tl_attn_bwd (below) with kv_start_dev as above, for the
+ * output of tl_attn_prefill_fwd_rows at past_len = 0 (k/v caches hold keys 0..S-1):
+ *   - the q, dout, out and lse rows of pad queries (s < kv_start[b]) and the K/V slots below kv_start[b] may hold
+ *     anything, NaN included; they are never read, or meet the backward through a select only;
+ *   - on exit dq is 0 on pad query rows and dk/dv are 0 on slots below kv_start[b]; every output is finite;
+ *   - with every kv_start[b] = 0 each result equals tl_attn_bwd's bit for bit.
+ * Dispatch is tl_attn_bwd's (wgmma kernels from S >= 64, mma.sync below; TL_ATTN_BWD=mma|wgmma forces a path). */
+int tl_attn_bwd_rows(const void* q, const void* k_cache, const void* v_cache, const void* out, const void* dout,
+                     const float* lse, void* dq, void* dk, void* dv, void* workspace, size_t ws_bytes, int B, int S,
+                     int n_h, int n_kv, int d, int T_max, float scale, const int32_t* kv_start_dev, void* stream);
 
 /* ---- K7  final norm + lm_head + greedy argmax for M <= 8 rows: ids[m] = argmax_v bf16(norm(x)[m,:]·W[v,:])
  * (lowest index wins ties, as torch.argmax).  logits_out (bf16 [M,V]) optional.

@@ -60,12 +60,15 @@ __global__ void attn_bwd_dot_kernel(const bf16* __restrict__ o, const bf16* __re
 }
 
 // ------------------------------------------------------------------------------------------------ pass 1: dQ
-template <int D>
+// ROWS: keys below kv_start[b] are pad slots.  A query tile made only of pad rows writes dq = 0 and loads nothing; the
+// KV loop starts at tile kv_start / 64, pad K/V rows load as zeros, and dS of pad keys (and so of pad query rows) is 0
+// by select: pad q, dO, lse and D may hold anything.
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dq_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k_cache,
                                                                   const bf16* __restrict__ v_cache, const bf16* __restrict__ dout,
                                                                   const float* __restrict__ lse, const float* __restrict__ Dv,
                                                                   bf16* __restrict__ dq, int S, int n_h, int n_kv, int T_max,
-                                                                  float scale) {
+                                                                  float scale, const int32_t* __restrict__ kv_start) {
     constexpr int LDS = D + 8, CPR = D / 8;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     bf16* sQ = reinterpret_cast<bf16*>(smem_raw);
@@ -79,6 +82,22 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dq_kernel(const bf16* __r
     const bf16* dog = dout + ((size_t)b * S) * n_h * D + (size_t)h * D;
     const bf16* kg = k_cache + ((size_t)b * n_kv + kvh) * T_max * D;
     const bf16* vg = v_cache + ((size_t)b * n_kv + kvh) * T_max * D;
+    int k_start = 0, t0 = 0;                               // first valid key and its tile
+    if constexpr (ROWS) {
+        k_start = kv_start[b];
+        if (min(S, q0 + AB_BQ) <= k_start) {               // every query row of this tile is a pad row
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int row = q0 + warp * 16 + g + r * 8;
+                if (row >= S) continue;
+                bf16* dst = dq + ((size_t)b * S + row) * n_h * D + (size_t)h * D;
+#pragma unroll
+                for (int i = 0; i < D / 8; ++i) *reinterpret_cast<uint32_t*>(dst + i * 8 + 2 * t4) = 0u;
+            }
+            return;
+        }
+        t0 = k_start / AB_BKV;
+    }
     for (int c = tid; c < AB_BQ * CPR; c += AB_THREADS) {
         const int r = c / CPR, cc = c - r * CPR;
         const bool ok = (q0 + r) < S;
@@ -89,14 +108,14 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dq_kernel(const bf16* __r
     auto load_kv = [&](int buf, int kv0) {
         for (int c = tid; c < AB_BKV * CPR; c += AB_THREADS) {
             const int r = c / CPR, cc = c - r * CPR;
-            const bool ok = (kv0 + r) < S;
+            const bool ok = (kv0 + r) < S && (!ROWS || (kv0 + r) >= k_start);   // pad slots load as zeros
             const size_t off = (size_t)(ok ? kv0 + r : 0) * D + cc * 8;
             cp16(sK + (buf * AB_BKV + r) * LDS + cc * 8, kg + off, ok);
             cp16(sV + (buf * AB_BKV + r) * LDS + cc * 8, vg + off, ok);
         }
     };
     const int n_tiles = (min(S, q0 + AB_BQ) + AB_BKV - 1) / AB_BKV;
-    load_kv(0, 0);
+    load_kv(0, t0 * AB_BKV);
     cp_commit();
     float acc[D / 8][4];
 #pragma unroll
@@ -111,8 +130,8 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dq_kernel(const bf16* __r
         dvr[r] = ok ? Dv[((size_t)b * n_h + h) * S + row] : 0.f;
     }
     const float sl2 = scale * LOG2E;
-    for (int it = 0; it < n_tiles; ++it) {
-        const int buf = it & 1;
+    for (int it = t0; it < n_tiles; ++it) {
+        const int buf = (it - t0) & 1;
         if (it + 1 < n_tiles) load_kv(buf ^ 1, (it + 1) * AB_BKV);
         cp_commit();
         cp_wait<1>();
@@ -153,8 +172,13 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dq_kernel(const bf16* __r
                 const int key = kv0 + i * 8 + 2 * t4 + (e & 1);
                 const int r = e >> 1;
                 const int qpos = row0 + r * 8;
-                const float p = (key > qpos || key >= S) ? 0.f : exp2f(s[i][e] * sl2 - lse2[r]);
-                ds[e] = p * (dp[i][e] - dvr[r]) * scale;
+                if constexpr (ROWS) {       // key >= k_start also masks pad query rows (key <= qpos < k_start)
+                    const bool ok = key <= qpos && key < S && key >= k_start;
+                    ds[e] = ok ? exp2f(s[i][e] * sl2 - lse2[r]) * (dp[i][e] - dvr[r]) * scale : 0.f;
+                } else {
+                    const float p = (key > qpos || key >= S) ? 0.f : exp2f(s[i][e] * sl2 - lse2[r]);
+                    ds[e] = p * (dp[i][e] - dvr[r]) * scale;
+                }
             }
             dsf[i >> 1][(i & 1) * 2] = pack_bf16(ds[0], ds[1]);
             dsf[i >> 1][(i & 1) * 2 + 1] = pack_bf16(ds[2], ds[3]);
@@ -184,12 +208,16 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dq_kernel(const bf16* __r
 }
 
 // ------------------------------------------------------------------------------------------------ pass 2: dK, dV
-template <int D>
+// ROWS: a key tile lying wholly below kv_start[b] writes dk = dv = 0 and loads nothing.  Pad K/V rows and the Q / dO
+// rows of pad queries load as zeros, and P / dS of pad keys and pad query rows are 0 by select, so pad key rows end as
+// exact zeros.
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dkv_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k_cache,
                                                                    const bf16* __restrict__ v_cache, const bf16* __restrict__ dout,
                                                                    const float* __restrict__ lse, const float* __restrict__ Dv,
                                                                    bf16* __restrict__ dk, bf16* __restrict__ dv, int S, int n_h,
-                                                                   int n_kv, int T_max, float scale) {
+                                                                   int n_kv, int T_max, float scale,
+                                                                   const int32_t* __restrict__ kv_start) {
     constexpr int LDS = D + 8, CPR = D / 8;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     bf16* sK = reinterpret_cast<bf16*>(smem_raw);      // [64][LDS]
@@ -205,9 +233,28 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dkv_kernel(const bf16* __
     const int n_rep = n_h / n_kv, kvh = h / n_rep, kv0 = kt * AB_BKV;
     const bf16* kg = k_cache + ((size_t)b * n_kv + kvh) * T_max * D;
     const bf16* vg = v_cache + ((size_t)b * n_kv + kvh) * T_max * D;
+    int k_start = 0;
+    if constexpr (ROWS) {
+        k_start = kv_start[b];
+        if (kv0 + AB_BKV <= k_start) {                     // every key of this tile is a pad slot
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int key = kv0 + warp * 16 + g + r * 8;
+                if (key >= S) continue;
+                bf16* dkd = dk + (((size_t)b * n_h + h) * T_max + key) * D;
+                bf16* dvd = dv + (((size_t)b * n_h + h) * T_max + key) * D;
+#pragma unroll
+                for (int i = 0; i < D / 8; ++i) {
+                    *reinterpret_cast<uint32_t*>(dkd + i * 8 + 2 * t4) = 0u;
+                    *reinterpret_cast<uint32_t*>(dvd + i * 8 + 2 * t4) = 0u;
+                }
+            }
+            return;
+        }
+    }
     for (int c = tid; c < AB_BKV * CPR; c += AB_THREADS) {
         const int r = c / CPR, cc = c - r * CPR;
-        const bool ok = (kv0 + r) < S;
+        const bool ok = (kv0 + r) < S && (!ROWS || (kv0 + r) >= k_start);   // pad slots load as zeros
         const size_t off = (size_t)(ok ? kv0 + r : 0) * D + cc * 8;
         cp16(sK + r * LDS + cc * 8, kg + off, ok);
         cp16(sV + r * LDS + cc * 8, vg + off, ok);
@@ -222,13 +269,13 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dkv_kernel(const bf16* __
         const bf16* dog = dout + ((size_t)b * S) * n_h * D + (size_t)h * D;
         for (int c = tid; c < AB_BQ * CPR; c += AB_THREADS) {
             const int r = c / CPR, cc = c - r * CPR;
-            const bool ok = (q0 + r) < S;
+            const bool ok = (q0 + r) < S && (!ROWS || (q0 + r) >= k_start);   // pad query rows load as zeros
             const size_t off = (size_t)(ok ? q0 + r : 0) * n_h * D + cc * 8;
             cp16(sQ + (buf * AB_BQ + r) * LDS + cc * 8, qg + off, ok);
             cp16(sdO + (buf * AB_BQ + r) * LDS + cc * 8, dog + off, ok);
         }
         if (tid < AB_BQ) {
-            const bool ok = (q0 + tid) < S;
+            const bool ok = (q0 + tid) < S && (!ROWS || (q0 + tid) >= k_start);
             const size_t idx = ((size_t)b * n_h + h) * S + (ok ? q0 + tid : 0);
             sL[buf * AB_BQ + tid] = ok ? lse[idx] * LOG2E : INFINITY;   // +inf -> P = 0 for padded queries
             sD[buf * AB_BQ + tid] = ok ? Dv[idx] : 0.f;
@@ -290,7 +337,9 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dkv_kernel(const bf16* __
                     const int qc = half * 32 + i * 8 + 2 * t4 + (e & 1);        // query column inside the tile
                     const int key = key_row0 + (e >> 1) * 8;
                     const int qpos = q0 + qc;
-                    p[e] = (key > qpos || key >= S) ? 0.f : exp2f(st[i][e] * sl2 - sLb[qc]);
+                    // ROWS: key >= k_start also masks pad query rows (key <= qpos < k_start); dS = P·(...) stays exact
+                    // zero there, every operand of a pad row or slot having loaded as zero (D as 0)
+                    p[e] = (key > qpos || key >= S || (ROWS && key < k_start)) ? 0.f : exp2f(st[i][e] * sl2 - sLb[qc]);
                     ds[e] = p[e] * (dpt[i][e] - sDb[qc]) * scale;
                 }
                 pf[i >> 1][(i & 1) * 2] = pack_bf16(p[0], p[1]);
@@ -334,23 +383,19 @@ __global__ void __launch_bounds__(AB_THREADS) attn_bwd_dkv_kernel(const bf16* __
 
 namespace tl {
 int attn_bwd_wgmma(const void* q, const void* k_cache, const void* v_cache, const void* dout, const float* lse, const float* Dv,
-                   void* dq, void* dk, void* dv, int B, int S, int n_h, int n_kv, int d, int T_max, float scale, cudaStream_t st);
-}
+                   void* dq, void* dk, void* dv, int B, int S, int n_h, int n_kv, int d, int T_max, float scale,
+                   const int32_t* kv_start, cudaStream_t st);
 
-extern "C" {
-
-size_t tl_attn_bwd_ws(int B, int S, int n_h) { return (size_t)B * n_h * S * sizeof(float); }
-
-int tl_attn_bwd(const void* q, const void* k_cache, const void* v_cache, const void* out, const void* dout, const float* lse,
-                void* dq, void* dk, void* dv, void* workspace, size_t ws_bytes, int B, int S, int n_h, int n_kv, int d,
-                int T_max, float scale, void* stream) {
-    using namespace tl;
-    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "tl_attn_bwd: head_dim %d not in {64,128}", d);
-    TL_REQUIRE(n_kv > 0 && n_h % n_kv == 0 && S <= T_max, TL_ERR_INVALID, "tl_attn_bwd: bad head/sequence configuration");
-    TL_REQUIRE(ws_bytes >= tl_attn_bwd_ws(B, S, n_h), TL_ERR_WORKSPACE, "tl_attn_bwd: workspace %zu < %zu", ws_bytes,
+// kv_start (int32[B], device) non-null: the left-padded instantiations (ROWS)
+static int attn_bwd_launch(const void* q, const void* k_cache, const void* v_cache, const void* out, const void* dout,
+                           const float* lse, void* dq, void* dk, void* dv, void* workspace, size_t ws_bytes, int B, int S,
+                           int n_h, int n_kv, int d, int T_max, float scale, const int32_t* kv_start, cudaStream_t st,
+                           const char* what) {
+    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "%s: head_dim %d not in {64,128}", what, d);
+    TL_REQUIRE(n_kv > 0 && n_h % n_kv == 0 && S <= T_max, TL_ERR_INVALID, "%s: bad head/sequence configuration", what);
+    TL_REQUIRE(ws_bytes >= tl_attn_bwd_ws(B, S, n_h), TL_ERR_WORKSPACE, "%s: workspace %zu < %zu", what, ws_bytes,
                tl_attn_bwd_ws(B, S, n_h));
     if (B == 0 || S == 0) return TL_OK;
-    cudaStream_t st = (cudaStream_t)stream;
     float* Dv = (float*)workspace;
     const long long total = (long long)B * S * n_h;
     const int g0 = (int)((total * 32 + 255) / 256);
@@ -361,37 +406,56 @@ int tl_attn_bwd(const void* q, const void* k_cache, const void* v_cache, const v
         if (impl == 2 || (impl == 0 && S >= AB_BQ)) {
             if (d == 64) attn_bwd_dot_kernel<64><<<g0, 256, 0, st>>>((const bf16*)out, (const bf16*)dout, Dv, S, n_h, total);
             else attn_bwd_dot_kernel<128><<<g0, 256, 0, st>>>((const bf16*)out, (const bf16*)dout, Dv, S, n_h, total);
-            return attn_bwd_wgmma(q, k_cache, v_cache, dout, lse, Dv, dq, dk, dv, B, S, n_h, n_kv, d, T_max, scale, st);
+            return attn_bwd_wgmma(q, k_cache, v_cache, dout, lse, Dv, dq, dk, dv, B, S, n_h, n_kv, d, T_max, scale, kv_start, st);
         }
     }
     const size_t sm1 = (size_t)6 * 64 * (d + 8) * sizeof(bf16);
     const size_t sm2 = (size_t)6 * 64 * (d + 8) * sizeof(bf16) + 4 * 64 * sizeof(float);
-    if (d == 64) {
-        static bool done = false;
-        if (!done) {
-            cudaFuncSetAttribute(attn_bwd_dq_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1);
-            cudaFuncSetAttribute(attn_bwd_dkv_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2);
-            done = true;
-        }
-        attn_bwd_dot_kernel<64><<<g0, 256, 0, st>>>((const bf16*)out, (const bf16*)dout, Dv, S, n_h, total);
-        attn_bwd_dq_kernel<64><<<g1, AB_THREADS, sm1, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                            (const bf16*)dout, lse, Dv, (bf16*)dq, S, n_h, n_kv, T_max, scale);
-        attn_bwd_dkv_kernel<64><<<g2, AB_THREADS, sm2, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                             (const bf16*)dout, lse, Dv, (bf16*)dk, (bf16*)dv, S, n_h, n_kv, T_max, scale);
+#define TL_AB_BWD(D_, ROWS_)                                                                                                \
+    do {                                                                                                                    \
+        static bool done = false;                                                                                           \
+        if (!done) {                                                                                                        \
+            cudaFuncSetAttribute(attn_bwd_dq_kernel<D_, ROWS_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1);      \
+            cudaFuncSetAttribute(attn_bwd_dkv_kernel<D_, ROWS_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2);     \
+            done = true;                                                                                                    \
+        }                                                                                                                   \
+        attn_bwd_dot_kernel<D_><<<g0, 256, 0, st>>>((const bf16*)out, (const bf16*)dout, Dv, S, n_h, total);                \
+        attn_bwd_dq_kernel<D_, ROWS_><<<g1, AB_THREADS, sm1, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache, \
+                                                                   (const bf16*)dout, lse, Dv, (bf16*)dq, S, n_h, n_kv,     \
+                                                                   T_max, scale, kv_start);                                 \
+        attn_bwd_dkv_kernel<D_, ROWS_><<<g2, AB_THREADS, sm2, st>>>((const bf16*)q, (const bf16*)k_cache,                   \
+                                                                    (const bf16*)v_cache, (const bf16*)dout, lse, Dv,       \
+                                                                    (bf16*)dk, (bf16*)dv, S, n_h, n_kv, T_max, scale,       \
+                                                                    kv_start);                                              \
+    } while (0)
+    if (kv_start) {
+        if (d == 64) TL_AB_BWD(64, true); else TL_AB_BWD(128, true);
     } else {
-        static bool done = false;
-        if (!done) {
-            cudaFuncSetAttribute(attn_bwd_dq_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm1);
-            cudaFuncSetAttribute(attn_bwd_dkv_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm2);
-            done = true;
-        }
-        attn_bwd_dot_kernel<128><<<g0, 256, 0, st>>>((const bf16*)out, (const bf16*)dout, Dv, S, n_h, total);
-        attn_bwd_dq_kernel<128><<<g1, AB_THREADS, sm1, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                             (const bf16*)dout, lse, Dv, (bf16*)dq, S, n_h, n_kv, T_max, scale);
-        attn_bwd_dkv_kernel<128><<<g2, AB_THREADS, sm2, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,
-                                                              (const bf16*)dout, lse, Dv, (bf16*)dk, (bf16*)dv, S, n_h, n_kv, T_max, scale);
+        if (d == 64) TL_AB_BWD(64, false); else TL_AB_BWD(128, false);
     }
-    return check_launch("tl_attn_bwd");
+#undef TL_AB_BWD
+    return check_launch(what);
+}
+}  // namespace tl
+
+extern "C" {
+
+size_t tl_attn_bwd_ws(int B, int S, int n_h) { return (size_t)B * n_h * S * sizeof(float); }
+
+int tl_attn_bwd(const void* q, const void* k_cache, const void* v_cache, const void* out, const void* dout, const float* lse,
+                void* dq, void* dk, void* dv, void* workspace, size_t ws_bytes, int B, int S, int n_h, int n_kv, int d,
+                int T_max, float scale, void* stream) {
+    return tl::attn_bwd_launch(q, k_cache, v_cache, out, dout, lse, dq, dk, dv, workspace, ws_bytes, B, S, n_h, n_kv, d,
+                               T_max, scale, nullptr, (cudaStream_t)stream, "tl_attn_bwd");
+}
+
+int tl_attn_bwd_rows(const void* q, const void* k_cache, const void* v_cache, const void* out, const void* dout,
+                     const float* lse, void* dq, void* dk, void* dv, void* workspace, size_t ws_bytes, int B, int S, int n_h,
+                     int n_kv, int d, int T_max, float scale, const int32_t* kv_start_dev, void* stream) {
+    using namespace tl;
+    TL_REQUIRE(kv_start_dev != nullptr, TL_ERR_INVALID, "tl_attn_bwd_rows: kv_start_dev is null");
+    return attn_bwd_launch(q, k_cache, v_cache, out, dout, lse, dq, dk, dv, workspace, ws_bytes, B, S, n_h, n_kv, d, T_max,
+                           scale, kv_start_dev, (cudaStream_t)stream, "tl_attn_bwd_rows");
 }
 
 }  // extern "C"

@@ -226,14 +226,17 @@ __global__ void __launch_bounds__(AW_THREADS) attn_fwd_wgmma_kernel(const __grid
 }
 
 // ================================================================================================ backward pass 1: dQ
-template <int D>
+// ROWS: keys below kv_start[b] are pad slots.  A query tile made only of pad rows writes dq = 0 and loads nothing; the
+// KV loop starts at tile kv_start / 64, the first tile's pad K/V rows are zeroed, and P / dS of pad keys (and so of pad
+// query rows, which see no key at or below them) are 0 by select: pad q, dO, lse and D may hold anything.
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dq_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ,
                                                                        const __grid_constant__ CUtensorMap tmdO,
                                                                        const __grid_constant__ CUtensorMap tmK,
                                                                        const __grid_constant__ CUtensorMap tmV,
                                                                        const float* __restrict__ lse, const float* __restrict__ Dv,
                                                                        bf16* __restrict__ dq, int S, int n_h, int n_kv, int T_max,
-                                                                       float scale) {
+                                                                       float scale, const int32_t* __restrict__ kv_start) {
     constexpr int TB = AwTile<D>::BYTES;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -245,16 +248,32 @@ __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dq_wgmma_kernel(const __g
     const int n_keys = min(S, q0 + AW_ROWS);
     const int n_tiles = (n_keys + AW_ROWS - 1) / AW_ROWS;
     const int kv_row = (b * n_kv + kvh) * T_max;
+    int k_start = 0, t0 = 0;                                  // first valid key and its tile
+    if constexpr (ROWS) {
+        k_start = kv_start[b];
+        if (n_keys <= k_start) {                              // every query row of this tile is a pad row
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int row = q0 + aw_row(0) + 8 * r;
+                if (row >= S) continue;
+                bf16* dst = dq + ((size_t)b * S + row) * n_h * D + (size_t)h * D;
+#pragma unroll
+                for (int i = 2 * r; i < D / 2; i += 4) *reinterpret_cast<uint32_t*>(dst + aw_col(i)) = 0u;
+            }
+            return;
+        }
+        t0 = k_start / AW_ROWS;
+    }
     if (threadIdx.x == 0) {
         for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
         fence_barrier_init();
         mbar_expect_tx(&bars[0], 2 * TB);
         aw_load<D>(sQ, &tmQ, &bars[0], b * S + q0, h * D);
         aw_load<D>(sdO, &tmdO, &bars[0], b * S + q0, h * D);
-        for (int t = 0; t < 2 && t < n_tiles; ++t) {
+        for (int t = 0; t < 2 && t0 + t < n_tiles; ++t) {
             mbar_expect_tx(&bars[1 + t], 2 * TB);
-            aw_load<D>(sK + t * 2 * TB, &tmK, &bars[1 + t], kv_row + t * AW_ROWS, 0);
-            aw_load<D>(sK + t * 2 * TB + TB, &tmV, &bars[1 + t], kv_row + t * AW_ROWS, 0);
+            aw_load<D>(sK + t * 2 * TB, &tmK, &bars[1 + t], kv_row + (t0 + t) * AW_ROWS, 0);
+            aw_load<D>(sK + t * 2 * TB + TB, &tmV, &bars[1 + t], kv_row + (t0 + t) * AW_ROWS, 0);
         }
     }
     const int row0 = q0 + aw_row(0);
@@ -272,13 +291,19 @@ __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dq_wgmma_kernel(const __g
 
     float acc[D / 2];
     aw_zero(acc);
-    for (int t = 0; t < n_tiles; ++t) {
-        const int slot = t & 1;
+    for (int t = t0; t < n_tiles; ++t) {
+        const int slot = (t - t0) & 1;
         unsigned char* k = sK + slot * 2 * TB;
         unsigned char* v = k + TB;
-        mbar_wait(&bars[1 + slot], (t >> 1) & 1);
+        mbar_wait(&bars[1 + slot], ((t - t0) >> 1) & 1);
         const int kv0 = t * AW_ROWS;
-        if (kv0 + AW_ROWS > S) {                         // keys past S: dS = 0 must meet finite K / V rows
+        if constexpr (ROWS) {
+            if (kv0 < k_start || kv0 + AW_ROWS > S) {         // pad slots and keys past S: dS = 0 must meet finite K / V
+                aw_zero_rows_outside<D>(k, k_start - kv0, S - kv0);
+                aw_zero_rows_outside<D>(v, k_start - kv0, S - kv0);
+                __syncthreads();
+            }
+        } else if (kv0 + AW_ROWS > S) {                  // keys past S: dS = 0 must meet finite K / V rows
             aw_zero_rows<D>(k, S - kv0);
             aw_zero_rows<D>(v, S - kv0);
             __syncthreads();
@@ -296,8 +321,13 @@ __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dq_wgmma_kernel(const __g
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
             const int key = kv0 + aw_col(i), r = (i >> 1) & 1;
-            const float p = (key > row0 + 8 * r || key >= S) ? 0.f : exp2f(s[i] * sl2 - lse2[r]);
-            s[i] = p * (dp[i] - dvr[r]) * scale;
+            if constexpr (ROWS) {       // key >= k_start also masks pad query rows (key <= row < k_start)
+                const bool ok = key <= row0 + 8 * r && key < S && key >= k_start;
+                s[i] = ok ? exp2f(s[i] * sl2 - lse2[r]) * (dp[i] - dvr[r]) * scale : 0.f;
+            } else {
+                const float p = (key > row0 + 8 * r || key >= S) ? 0.f : exp2f(s[i] * sl2 - lse2[r]);
+                s[i] = p * (dp[i] - dvr[r]) * scale;
+            }
         }
         uint32_t dsf[4][4];
         aw_frag(s, dsf);
@@ -325,14 +355,18 @@ __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dq_wgmma_kernel(const __g
 }
 
 // ================================================================================================ backward pass 2: dK, dV
-template <int D>
+// ROWS: a key tile lying wholly below kv_start[b] writes dk = dv = 0 and loads nothing.  P / dS of pad keys and pad
+// query rows are 0 by select, and the Q / dO rows of a query tile outside [kv_start, S) are zeroed before they meet
+// P^T / dS^T (rows past S belong to the next batch row and may be its pad rows), so pad key rows end as exact zeros.
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dkv_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ,
                                                                         const __grid_constant__ CUtensorMap tmdO,
                                                                         const __grid_constant__ CUtensorMap tmK,
                                                                         const __grid_constant__ CUtensorMap tmV,
                                                                         const float* __restrict__ lse, const float* __restrict__ Dv,
                                                                         bf16* __restrict__ dk, bf16* __restrict__ dv, int S, int n_h,
-                                                                        int n_kv, int T_max, float scale) {
+                                                                        int n_kv, int T_max, float scale,
+                                                                        const int32_t* __restrict__ kv_start) {
     constexpr int TB = AwTile<D>::BYTES;
     extern __shared__ unsigned char smem_dyn[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -343,6 +377,25 @@ __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dkv_wgmma_kernel(const __
     const int k0 = blockIdx.x * AW_ROWS, h = blockIdx.y, b = blockIdx.z, kvh = h / (n_h / n_kv);
     const int qt0 = blockIdx.x, n_tiles = (S + AW_ROWS - 1) / AW_ROWS - qt0;   // query tiles at or after this key tile
     const int kv_row = (b * n_kv + kvh) * T_max;
+    int k_start = 0;
+    if constexpr (ROWS) {
+        k_start = kv_start[b];
+        if (k0 + AW_ROWS <= k_start) {                        // every key of this tile is a pad slot
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int key = k0 + aw_row(0) + 8 * r;
+                if (key >= S) continue;
+                bf16* dkd = dk + (((size_t)b * n_h + h) * T_max + key) * D;
+                bf16* dvd = dv + (((size_t)b * n_h + h) * T_max + key) * D;
+#pragma unroll
+                for (int i = 2 * r; i < D / 2; i += 4) {
+                    *reinterpret_cast<uint32_t*>(dkd + aw_col(i)) = 0u;
+                    *reinterpret_cast<uint32_t*>(dvd + aw_col(i)) = 0u;
+                }
+            }
+            return;
+        }
+    }
     if (threadIdx.x == 0) {
         for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
         fence_barrier_init();
@@ -371,6 +424,13 @@ __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dkv_wgmma_kernel(const __
         unsigned char* dot = qt + TB;
         mbar_wait(&bars[1 + slot], (t >> 1) & 1);
         const int qb = (qt0 + t) * AW_ROWS;
+        if constexpr (ROWS) {
+            if (qb < k_start || qb + AW_ROWS > S) {           // pad query rows and rows past S: P^T·dO, dS^T·Q see zeros
+                aw_zero_rows_outside<D>(qt, k_start - qb, S - qb);
+                aw_zero_rows_outside<D>(dot, k_start - qb, S - qb);
+                __syncthreads();
+            }
+        }
         float st[32], dpt[32];
         wgmma_fence_acc(st);
         wgmma_fence_acc(dpt);
@@ -384,7 +444,7 @@ __global__ void __launch_bounds__(AW_THREADS) attn_bwd_dkv_wgmma_kernel(const __
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
             const int qpos = qb + aw_col(i), key = key0 + 8 * ((i >> 1) & 1);
-            const bool ok = qpos < S && key <= qpos;
+            const bool ok = qpos < S && key <= qpos && (!ROWS || key >= k_start);
             const int qc = min(qpos, S - 1);
             const float p = ok ? exp2f(st[i] * sl2 - lse_bh[qc] * AW_LOG2E) : 0.f;
             st[i] = p;
@@ -457,9 +517,10 @@ int attn_prefill_wgmma(const void* q, const void* k_cache, const void* v_cache, 
     return check_launch("tl_attn_prefill_fwd (wgmma)");
 }
 
-// Dv (rowsum dO·O) must already be in place
+// Dv (rowsum dO·O) must already be in place; kv_start (int32[B], device) non-null: the left-padded instantiations (ROWS)
 int attn_bwd_wgmma(const void* q, const void* k_cache, const void* v_cache, const void* dout, const float* lse, const float* Dv,
-                   void* dq, void* dk, void* dv, int B, int S, int n_h, int n_kv, int d, int T_max, float scale, cudaStream_t st) {
+                   void* dq, void* dk, void* dv, int B, int S, int n_h, int n_kv, int d, int T_max, float scale,
+                   const int32_t* kv_start, cudaStream_t st) {
     CUtensorMap tq, tdo, tk, tv;
     int rc = make_tensor_map(&tq, q, (uint64_t)n_h * d, (uint64_t)B * S, (uint64_t)n_h * d, 64, 64);
     if (rc == TL_OK) rc = make_tensor_map(&tdo, dout, (uint64_t)n_h * d, (uint64_t)B * S, (uint64_t)n_h * d, 64, 64);
@@ -467,21 +528,22 @@ int attn_bwd_wgmma(const void* q, const void* k_cache, const void* v_cache, cons
     if (rc == TL_OK) rc = make_tensor_map(&tv, v_cache, d, (uint64_t)B * n_kv * T_max, d, 64, 64);
     if (rc != TL_OK) return rc;
     const dim3 grid((S + AW_ROWS - 1) / AW_ROWS, n_h, B);
-    if (d == 64) {
-        const int smem = 6 * AwTile<64>::BYTES + 1024 + 64;
-        aw_smem_attr<64, 1>((const void*)attn_bwd_dq_wgmma_kernel<64>, smem);
-        aw_smem_attr<64, 2>((const void*)attn_bwd_dkv_wgmma_kernel<64>, smem);
-        attn_bwd_dq_wgmma_kernel<64><<<grid, AW_THREADS, smem, st>>>(tq, tdo, tk, tv, lse, Dv, (bf16*)dq, S, n_h, n_kv, T_max, scale);
-        attn_bwd_dkv_wgmma_kernel<64><<<grid, AW_THREADS, smem, st>>>(tq, tdo, tk, tv, lse, Dv, (bf16*)dk, (bf16*)dv, S, n_h, n_kv,
-                                                                       T_max, scale);
+#define TL_AW_BWD(D_, ROWS_, WHICH_)                                                                                        \
+    do {                                                                                                                    \
+        const int smem = 6 * AwTile<D_>::BYTES + 1024 + 64;                                                                 \
+        aw_smem_attr<D_, WHICH_>((const void*)attn_bwd_dq_wgmma_kernel<D_, ROWS_>, smem);                                   \
+        aw_smem_attr<D_, WHICH_ + 1>((const void*)attn_bwd_dkv_wgmma_kernel<D_, ROWS_>, smem);                              \
+        attn_bwd_dq_wgmma_kernel<D_, ROWS_><<<grid, AW_THREADS, smem, st>>>(tq, tdo, tk, tv, lse, Dv, (bf16*)dq, S, n_h, n_kv, \
+                                                                            T_max, scale, kv_start);                        \
+        attn_bwd_dkv_wgmma_kernel<D_, ROWS_><<<grid, AW_THREADS, smem, st>>>(tq, tdo, tk, tv, lse, Dv, (bf16*)dk, (bf16*)dv,  \
+                                                                             S, n_h, n_kv, T_max, scale, kv_start);         \
+    } while (0)
+    if (kv_start) {
+        if (d == 64) TL_AW_BWD(64, true, 4); else TL_AW_BWD(128, true, 4);
     } else {
-        const int smem = 6 * AwTile<128>::BYTES + 1024 + 64;
-        aw_smem_attr<128, 1>((const void*)attn_bwd_dq_wgmma_kernel<128>, smem);
-        aw_smem_attr<128, 2>((const void*)attn_bwd_dkv_wgmma_kernel<128>, smem);
-        attn_bwd_dq_wgmma_kernel<128><<<grid, AW_THREADS, smem, st>>>(tq, tdo, tk, tv, lse, Dv, (bf16*)dq, S, n_h, n_kv, T_max, scale);
-        attn_bwd_dkv_wgmma_kernel<128><<<grid, AW_THREADS, smem, st>>>(tq, tdo, tk, tv, lse, Dv, (bf16*)dk, (bf16*)dv, S, n_h, n_kv,
-                                                                        T_max, scale);
+        if (d == 64) TL_AW_BWD(64, false, 1); else TL_AW_BWD(128, false, 1);
     }
+#undef TL_AW_BWD
     return check_launch("tl_attn_bwd (wgmma)");
 }
 

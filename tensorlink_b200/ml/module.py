@@ -82,6 +82,29 @@ def _check_attention_mask(mask, shape):
                                   "equal length")
 
 
+def _train_mask(mask, shape):
+    """A training batch's ``attention_mask`` as (kv_start, real): ``kv_start[b]`` is the number of leading pad tokens of
+    row b and ``real`` (bool [B,S], on the host) marks its real tokens; None when the mask has no zero.  Each row's ones
+    must form one run of at least one token (left, right or both sides padded): holes raise NotImplementedError, an
+    empty row or a mask shaped unlike ``input_ids`` raises ValueError."""
+    if mask is None:
+        return None
+    if tuple(mask.shape) != tuple(shape):
+        raise ValueError(f"attention_mask shape {tuple(mask.shape)} != input_ids shape {tuple(shape)}")
+    real = (mask != 0).cpu()
+    if bool(real.all()):
+        return None
+    lengths = real.sum(1)
+    if int(lengths.min()) == 0:
+        raise ValueError("attention_mask has a row without any real token")
+    starts = real.long().argmax(1)
+    cols = torch.arange(real.shape[1])[None, :]
+    if not torch.equal(real, (cols >= starts[:, None]) & (cols < (starts + lengths)[:, None])):
+        raise NotImplementedError("attention_mask rows must be one run of ones (padding on the left and/or the right, "
+                                  "no holes)")
+    return [int(v) for v in starts.tolist()], real
+
+
 def _left_pad_groups(mask: torch.Tensor):
     """A left-padded batch (HF's convention for generation: ``tokenizer(..., padding=True, padding_side='left')``)
     as {real length: [row indices]}; None when no row is padded.  Right padding / holes raise."""
@@ -277,19 +300,24 @@ class DistributedModel(torch.nn.Module):
     # ------------------------------------------------------------------------------------------ forward
     def forward(self, *args, **kwargs) -> CausalLMOutput:
         """One forward through every stage (module.py:348-407).  ``input_ids`` positional or keyword (:355-359).
-        Inference: logits [B,S,V] on the last stage.  Training (``self.training`` with a grad-enabled stage):
-        handled by ``ml/train.py``."""
+        Inference: logits [B,S,V] on the last stage, rows of equal length only.  Training (``self.training`` with a
+        grad-enabled stage): handled by ``ml/train.py``; a padded ``attention_mask`` is accepted there
+        (``train_forward``)."""
         input_ids = kwargs.pop("input_ids", args[0] if args else None)
         labels = kwargs.pop("labels", None)
         gather = kwargs.pop("gather_logits", False)
+        mask = kwargs.pop("attention_mask", None)
+        training = self.training and getattr(self.stage, "supports_training", False)
+        padding = None
         if self.link.first and input_ids is not None:
-            _check_attention_mask(kwargs.pop("attention_mask", None), input_ids.shape)
-        else:
-            kwargs.pop("attention_mask", None)
+            if training:
+                padding = _train_mask(mask, input_ids.shape)
+            else:
+                _check_attention_mask(mask, input_ids.shape)
         _check_unconsumed(kwargs, "DistributedModel.forward")
-        if self.training and getattr(self.stage, "supports_training", False):
+        if training:
             from .train import train_forward
-            return train_forward(self, input_ids, labels)
+            return train_forward(self, input_ids, labels, padding)
         return self._infer_forward(input_ids, gather)
 
     def _infer_forward(self, input_ids: Optional[torch.Tensor], gather: bool) -> CausalLMOutput:

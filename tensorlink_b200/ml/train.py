@@ -22,7 +22,7 @@ rank before the optimizer step, so both copies take identical updates.
 from __future__ import annotations
 
 import os
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -47,7 +47,12 @@ class StageTrainer:
     of the pipeline: a stage that has finished its dgrads fills the drain of the pipeline with its weight gradients
     (the "deferred W" of zero-bubble schedules) while earlier stages are still receiving gradients.
     As soon as a layer's gradients are final an event is recorded, so the optimizer can update that layer on a side
-    stream while the remaining weight-gradient GEMMs still run (``StageAdam.step``)."""
+    stream while the remaining weight-gradient GEMMs still run (``StageAdam.step``).
+
+    Left-padded micro-batches (``kv_start``, see ``train_forward``) run the ``_rows`` attention forward and backward:
+    keys below a row's start are never attended and pad tokens receive exact zeros from the attention backward."""
+
+    supports_kv_start = True
 
     def __init__(self, stage):
         self.st = stage
@@ -154,8 +159,10 @@ class StageTrainer:
         return torch.empty(b, S, self.cfg.hidden, dtype=torch.bfloat16, device=self.p.device)
 
     # ------------------------------------------------------------------------------------------ forward
-    def forward_layers(self, mb, x: torch.Tensor) -> torch.Tensor:
-        """x [b,S,H] -> [b,S,H] through this stage's layers, saving what the backward needs."""
+    def forward_layers(self, mb, x: torch.Tensor, kv_start: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """x [b,S,H] -> [b,S,H] through this stage's layers, saving what the backward needs.  ``kv_start`` (int32[b] on
+        the device, optional): leading pad tokens of each row, whose keys no query attends to (RoPE positions stay
+        0..S-1 in every row, as in HF's training forward)."""
         cfg, v = self.cfg, self.p.v
         b, S, H = x.shape
         N = b * S
@@ -180,7 +187,7 @@ class StageTrainer:
             s["attn"] = st["attn"][rows] if st else torch.empty(N, cfg.q_dim, dtype=bf, device=dev)
             s["lse"] = torch.empty(b, cfg.n_heads, S, dtype=torch.float32, device=dev)
             nat.attn_prefill_fwd(s["q"], s["kc"], s["vc"], s["attn"], s["lse"], b, S, 0, cfg.n_heads, cfg.n_kv_heads,
-                                 cfg.head_dim, self.grp.scale)
+                                 cfg.head_dim, self.grp.scale, kv_start=kv_start)
             s["x_mid"] = nat.gemm(s["attn"], v[f"l{li}.wo"], residual=x)
             s["rstd2"] = torch.empty(N, dtype=torch.float32, device=dev)
             s["h2"] = nat.rmsnorm_fwd(s["x_mid"], v[f"l{li}.ln2"], cfg.rms_eps, rstd=s["rstd2"], out=st["h2"][rows] if st else None)
@@ -190,7 +197,7 @@ class StageTrainer:
             x = nat.gemm(s["act"], v[f"l{li}.wd"], residual=s["x_mid"])
             saved.append(s)
             self.launches += 10
-        self.ctx[mb] = {"layers": saved, "b": b, "S": S, "deferred": rows is not None}
+        self.ctx[mb] = {"layers": saved, "b": b, "S": S, "deferred": rows is not None, "kv_start": kv_start}
         return x.view(b, S, H)
 
     def head_loss_and_grad(self, mb, x: torch.Tensor, shift_labels: torch.Tensor, inv_n: float) -> None:
@@ -319,7 +326,7 @@ class StageTrainer:
             dk = torch.empty(b, cfg.n_heads, S, cfg.head_dim, dtype=bf, device=dev)     # one partial per query head
             dv = torch.empty_like(dk)
             nat.attn_bwd(s["q"], s["kc"], s["vc"], s["attn"], d_attn, s["lse"], dq, dk, dv, ws, b, S, cfg.n_heads,
-                         cfg.n_kv_heads, cfg.head_dim, self.grp.scale)
+                         cfg.n_kv_heads, cfg.head_dim, self.grp.scale, kv_start=c.get("kv_start"))
             dqkv = st["dqkv"][rows] if st else torch.empty(N, cfg.qkv_dim, dtype=bf, device=dev)
             nat.rope_kv_bwd(dq, dk, dv, dqkv, self.grp.cos, self.grp.sin, S, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim)
             if cfg.qk_norm:
@@ -439,8 +446,19 @@ def _trainer(dm) -> StageTrainer:
     return dm.stage.trainer
 
 
-def train_forward(dm, input_ids: Optional[torch.Tensor], labels: Optional[torch.Tensor]) -> CausalLMOutput:
-    """Forward of all micro-batches (GPipe order).  Every rank returns an autograd proxy as ``.loss``."""
+def train_forward(dm, input_ids: Optional[torch.Tensor], labels: Optional[torch.Tensor],
+                  padding: Optional[Tuple[List[int], torch.Tensor]] = None) -> CausalLMOutput:
+    """Forward of all micro-batches (GPipe order).  Every rank returns an autograd proxy as ``.loss``.
+
+    ``padding`` (first rank; ``module._train_mask`` of the ``attention_mask``): (kv_start, real) of a padded batch.
+    A real query attends to the real keys of its row at or before it; RoPE positions stay 0..S-1 in every row, as in
+    HF's forward without ``position_ids``.  Left padding masks keys below ``kv_start[b]`` in the attention kernels;
+    right padding needs no kernel change (the causal mask already hides those keys from real queries).
+    Deviation from HF: every label predicted FROM a pad position is ignored (the shifted label at t becomes -100
+    where ``attention_mask[b, t] == 0``).  For right padding that is what collators already write; for left padding it
+    drops one term per row, the first real token predicted from the last pad, whose HF logits come from a fully
+    masked query row and differ between HF's attention backends.  Pad positions then carry no loss and real positions
+    never read them, so pad tokens get exactly zero gradient."""
     link, st, cfg, dev = dm.link, dm.stage, dm.cfg, dm.device
     tr = _trainer(dm)
     meta = None
@@ -449,8 +467,16 @@ def train_forward(dm, input_ids: Optional[torch.Tensor], labels: Optional[torch.
             raise ValueError("training forward needs labels= (the loss is produced on the last stage)")
         B, S = input_ids.shape
         shift = F.pad(labels, (0, 1), value=-100)[:, 1:].contiguous()
-        meta = (B, S, int((shift != -100).sum()))
-    B, S, n_valid = link.broadcast_object(meta)
+        starts = None
+        if padding is not None:
+            starts, real = padding
+            shift = shift.masked_fill(~real.to(shift.device), -100)
+            if not any(starts):
+                starts = None                    # right padding only: the plain kernels, exactly as an unpadded batch
+        meta = (B, S, int((shift != -100).sum()), starts)
+    B, S, n_valid, starts = link.broadcast_object(meta)
+    if starts is not None and not getattr(tr, "supports_kv_start", False):
+        raise NotImplementedError("left-padded training batches need a stage trainer with per-row key starts")
     n_mb = min(dm.n_pipelines, B)
     if B % n_mb:
         raise ValueError(f"batch {B} not divisible into {n_mb} micro-batches")
@@ -473,7 +499,11 @@ def train_forward(dm, input_ids: Optional[torch.Tensor], labels: Optional[torch.
         else:
             x = torch.empty(b, S, cfg.hidden, dtype=torch.bfloat16, device=dev)
             link.recv_prev(x)
-        x = tr.forward_layers(m, x)
+        mb_starts = starts[m * b:(m + 1) * b] if starts is not None else None
+        if mb_starts is not None and any(mb_starts):
+            x = tr.forward_layers(m, x, kv_start=torch.tensor(mb_starts, dtype=torch.int32, device=dev))
+        else:
+            x = tr.forward_layers(m, x)
         if not link.last:
             link.send_next(x.contiguous())
         else:

@@ -84,6 +84,8 @@ _SIGS = {
     "tl_qk_norm_bwd": (c_int, [c_void_p] * 6 + [c_float, c_int, c_int, c_int, c_int, c_void_p]),
     "tl_attn_bwd_ws": (c_size_t, [c_int, c_int, c_int]),
     "tl_attn_bwd": (c_int, [c_void_p] * 10 + [c_size_t, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+    "tl_attn_bwd_rows": (c_int, [c_void_p] * 10 + [c_size_t, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
+                                                   c_void_p]),
     "tl_ce_fwd_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_void_p]),
     "tl_embed_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "tl_colsum": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
@@ -481,11 +483,18 @@ def attn_bwd_ws(B, S, n_h) -> int:
     return int(load().tl_attn_bwd_ws(B, S, n_h))
 
 
-def attn_bwd(q, k_cache, v_cache, out, dout, lse, dq, dk, dv, ws, B, S, n_h, n_kv, d, scale):
+def attn_bwd(q, k_cache, v_cache, out, dout, lse, dq, dk, dv, ws, B, S, n_h, n_kv, d, scale, kv_start=None):
+    """``kv_start`` (int32[B] device, optional): left-padded rows, through ``tl_attn_bwd_rows``."""
     require_device(); _bf16(q, k_cache, v_cache, out, dout, dq, dk, dv)
-    _check(load().tl_attn_bwd(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(dout), _p(lse), _p(dq), _p(dk), _p(dv), _p(ws),
-                              ws.numel() * ws.element_size(), B, S, n_h, n_kv, d, k_cache.shape[2], scale, _stream()),
-           "tl_attn_bwd")
+    if kv_start is None:
+        _check(load().tl_attn_bwd(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(dout), _p(lse), _p(dq), _p(dk), _p(dv), _p(ws),
+                                  ws.numel() * ws.element_size(), B, S, n_h, n_kv, d, k_cache.shape[2], scale, _stream()),
+               "tl_attn_bwd")
+        return
+    _kv_start(kv_start, B)
+    _check(load().tl_attn_bwd_rows(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(dout), _p(lse), _p(dq), _p(dk), _p(dv),
+                                   _p(ws), ws.numel() * ws.element_size(), B, S, n_h, n_kv, d, k_cache.shape[2], scale,
+                                   _p(kv_start), _stream()), "tl_attn_bwd_rows")
 
 
 def ce_fwd_bwd(logits, labels, loss_sum, n_valid, dlogits, grad_scale: float):
