@@ -72,7 +72,7 @@ size_t tl_gemm_splitk_ws(int M, int N);
 int tl_gemm_bf16_ws(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                     const void* bias, const void* residual, int flags, void* workspace, size_t ws_bytes, void* stream);
 /* ... and the RMSNorm that follows this Linear in the decoder layer (modeling_qwen2.py:296 / :280 of the next layer):
- * with norm_w != NULL also writes H_out[M,N] = norm_w * bf16(C * rstd(C)), C being the bf16 result above (ldc == N,
+ * with norm_w != NULL also writes H_out[M,N] = norm_w * bf16(C * rstd(C)), C being the bf16 result above (ldc == N <= 8192,
  * bias / residual epilogue only).  Fused into the split-K reduce pass when that path runs, otherwise one extra
  * tl_rmsnorm_fwd launch (C identical either way; H may differ in a last bf16 bit: the row's sum of squares is reduced
  * in another order). */

@@ -443,6 +443,27 @@ splitk_reduce_norm_kernel(const float* __restrict__ ws, bf16* __restrict__ C, in
     }
 }
 
+// The argument checks of tl_gemm_bf16, made by tl_gemm_bf16_ws_norm too before it chooses the split-K path, which
+// would otherwise accept (and silently mis-execute) a combination tl_gemm_bf16 rejects.
+static int check_gemm_args(int M, int N, int K, int lda, int ldb, int ldc, const void* bias, const void* residual, int flags) {
+    TL_REQUIRE(M > 0 && N > 0 && K > 0, TL_ERR_INVALID, "tl_gemm_bf16: empty problem M=%d N=%d K=%d", M, N, K);
+    TL_REQUIRE(N % 8 == 0, TL_ERR_INVALID, "tl_gemm_bf16: N must be a multiple of 8 (N=%d)", N);
+    TL_REQUIRE(K % 8 == 0 || ((flags & TL_A_MN_MAJOR) && (flags & TL_B_MN_MAJOR)), TL_ERR_INVALID,
+               "tl_gemm_bf16: K must be a multiple of 8 for K-major operands (K=%d)", K);
+    TL_REQUIRE(!(flags & TL_EPI_BIAS) || bias, TL_ERR_INVALID, "tl_gemm_bf16: BIAS flag without bias pointer");
+    TL_REQUIRE(!(flags & TL_EPI_RESIDUAL) || residual, TL_ERR_INVALID, "tl_gemm_bf16: RESIDUAL flag without pointer");
+    const bool swiglu = flags & TL_EPI_SWIGLU;
+    TL_REQUIRE(!swiglu || !(flags & (TL_EPI_RESIDUAL | TL_EPI_OUT_F32 | TL_EPI_ACCUM)), TL_ERR_INVALID,
+               "tl_gemm_bf16: SWIGLU excludes RESIDUAL/OUT_F32/ACCUM");
+    TL_REQUIRE(!swiglu || N % 16 == 0, TL_ERR_INVALID, "tl_gemm_bf16: SWIGLU needs N %% 16 == 0");
+    const int c_cols = swiglu ? N / 2 : N;
+    TL_REQUIRE(ldc >= c_cols && ldc % 8 == 0, TL_ERR_INVALID, "tl_gemm_bf16: ldc=%d too small / unaligned", ldc);
+    const bool a_mn = flags & TL_A_MN_MAJOR, b_mn = flags & TL_B_MN_MAJOR;
+    TL_REQUIRE(lda >= (a_mn ? M : K) && ldb >= (b_mn ? N : K), TL_ERR_INVALID, "tl_gemm_bf16: lda/ldb too small");
+    TL_REQUIRE((!a_mn || M % 8 == 0), TL_ERR_INVALID, "tl_gemm_bf16: MN-major A needs M %% 8 == 0");
+    return TL_OK;
+}
+
 }  // namespace tl
 
 extern "C" size_t tl_gemm_splitk_ws(int M, int N) { return (size_t)8 * (size_t)(M > 128 ? 0 : M) * (size_t)N * sizeof(float); }
@@ -463,14 +484,20 @@ extern "C" int tl_gemm_bf16_ws(const void* A, const void* B, void* C, int M, int
                                 stream);
 }
 
-// ... and, when norm_w != NULL, H_out[M,N] = RMSNorm(C) * norm_w (the norm that follows this Linear in the decoder layer):
-// fused into the split-K reduce pass when that path is taken, a separate tl_rmsnorm_fwd launch otherwise (same bits).
+// ... and, when norm_w != NULL, H_out[M,N] = RMSNorm(C) * norm_w (the norm that follows this Linear in the decoder layer,
+// N <= 8192): fused into the split-K reduce pass when that path is taken, a separate tl_rmsnorm_fwd launch otherwise.
 extern "C" int tl_gemm_bf16_ws_norm(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                                     const void* bias, const void* residual, int flags, void* workspace, size_t ws_bytes,
                                     const void* norm_w, float eps, void* H_out, void* stream) {
     using namespace tl;
     TL_REQUIRE(!norm_w || (H_out && ldc == N && !(flags & (TL_EPI_SWIGLU | TL_EPI_OUT_F32 | TL_EPI_ACCUM))), TL_ERR_INVALID,
                "tl_gemm_bf16_ws_norm: the fused norm needs H_out, ldc == N and a plain bf16 (bias/residual) epilogue");
+    // both norm passes (the fused reduce and tl_rmsnorm_fwd) hold a whole row in registers: reject wider rows before
+    // anything is launched, rather than after C has been written
+    TL_REQUIRE(!norm_w || N <= RN_THREADS * RN_MAXV * 8, TL_ERR_INVALID, "tl_gemm_bf16_ws_norm: the fused norm needs N <= %d (N=%d)",
+               RN_THREADS * RN_MAXV * 8, N);
+    const int arg_rc = check_gemm_args(M, N, K, lda, ldb, ldc, bias, residual, flags);
+    if (arg_rc != TL_OK) return arg_rc;
     const int tiles_n = (N + 127) / 128, num_k = (K + BK - 1) / BK;
     const bool plain = !(flags & (TL_A_MN_MAJOR | TL_B_MN_MAJOR));
     if (workspace && plain && M > 0 && M <= BM && K % 8 == 0 && N % 8 == 0 && tiles_n * 2 <= sm_count() && num_k >= 16) {
@@ -480,13 +507,11 @@ extern "C" int tl_gemm_bf16_ws_norm(const void* A, const void* B, void* C, int M
         if (kb_per < 8) kb_per = 8;
         splits = (num_k + kb_per - 1) / kb_per;
         if (splits > 1 && ws_bytes >= (size_t)splits * M * N * sizeof(float)) {
-            TL_REQUIRE(!(flags & TL_EPI_BIAS) || bias, TL_ERR_INVALID, "tl_gemm_bf16_ws: BIAS flag without bias pointer");
-            TL_REQUIRE(!(flags & TL_EPI_RESIDUAL) || residual, TL_ERR_INVALID, "tl_gemm_bf16_ws: RESIDUAL flag without pointer");
             cudaStream_t st = (cudaStream_t)stream;
             int rc = launch_gemm<128, false, false>(A, B, workspace, M, N, K, lda, ldb, N, nullptr, nullptr, TL_EPI_OUT_F32, st,
                                                     splits, kb_per);
             if (rc != TL_OK) return rc;
-            if (norm_w && N <= RN_THREADS * RN_MAXV * 8) {
+            if (norm_w) {
                 splitk_reduce_norm_kernel<<<M, RN_THREADS, 0, st>>>((const float*)workspace, (bf16*)C, M, N, ldc, splits,
                                                                     (const bf16*)bias, (const bf16*)residual, ldc, flags,
                                                                     (const bf16*)norm_w, eps, (bf16*)H_out);
@@ -495,9 +520,7 @@ extern "C" int tl_gemm_bf16_ws_norm(const void* A, const void* B, void* C, int M
             const long long items = (long long)M * (N >> 3);
             splitk_reduce_kernel<<<(unsigned)((items + 255) / 256), 256, 0, st>>>((const float*)workspace, C, M, N, ldc, splits,
                                                                                   (const bf16*)bias, (const bf16*)residual, ldc, flags);
-            int rc2 = check_launch("tl_gemm_bf16_ws (reduce)");
-            if (rc2 != TL_OK || !norm_w) return rc2;
-            return tl_rmsnorm_fwd(C, norm_w, H_out, nullptr, M, N, eps, stream);
+            return check_launch("tl_gemm_bf16_ws (reduce)");
         }
     }
     int rc = tl_gemm_bf16(A, B, C, M, N, K, lda, ldb, ldc, bias, residual, flags, stream);
@@ -508,21 +531,9 @@ extern "C" int tl_gemm_bf16_ws_norm(const void* A, const void* B, void* C, int M
 extern "C" int tl_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
                             const void* bias, const void* residual, int flags, void* stream) {
     using namespace tl;
-    TL_REQUIRE(M > 0 && N > 0 && K > 0, TL_ERR_INVALID, "tl_gemm_bf16: empty problem M=%d N=%d K=%d", M, N, K);
-    TL_REQUIRE(N % 8 == 0, TL_ERR_INVALID, "tl_gemm_bf16: N must be a multiple of 8 (N=%d)", N);
-    TL_REQUIRE(K % 8 == 0 || ((flags & TL_A_MN_MAJOR) && (flags & TL_B_MN_MAJOR)), TL_ERR_INVALID,
-               "tl_gemm_bf16: K must be a multiple of 8 for K-major operands (K=%d)", K);
-    TL_REQUIRE(!(flags & TL_EPI_BIAS) || bias, TL_ERR_INVALID, "tl_gemm_bf16: BIAS flag without bias pointer");
-    TL_REQUIRE(!(flags & TL_EPI_RESIDUAL) || residual, TL_ERR_INVALID, "tl_gemm_bf16: RESIDUAL flag without pointer");
-    const bool swiglu = flags & TL_EPI_SWIGLU;
-    TL_REQUIRE(!swiglu || !(flags & (TL_EPI_RESIDUAL | TL_EPI_OUT_F32 | TL_EPI_ACCUM)), TL_ERR_INVALID,
-               "tl_gemm_bf16: SWIGLU excludes RESIDUAL/OUT_F32/ACCUM");
-    TL_REQUIRE(!swiglu || N % 16 == 0, TL_ERR_INVALID, "tl_gemm_bf16: SWIGLU needs N %% 16 == 0");
-    const int c_cols = swiglu ? N / 2 : N;
-    TL_REQUIRE(ldc >= c_cols && ldc % 8 == 0, TL_ERR_INVALID, "tl_gemm_bf16: ldc=%d too small / unaligned", ldc);
+    const int rc = check_gemm_args(M, N, K, lda, ldb, ldc, bias, residual, flags);
+    if (rc != TL_OK) return rc;
     const bool a_mn = flags & TL_A_MN_MAJOR, b_mn = flags & TL_B_MN_MAJOR;
-    TL_REQUIRE(lda >= (a_mn ? M : K) && ldb >= (b_mn ? N : K), TL_ERR_INVALID, "tl_gemm_bf16: lda/ldb too small");
-    TL_REQUIRE((!a_mn || M % 8 == 0), TL_ERR_INVALID, "tl_gemm_bf16: MN-major A needs M %% 8 == 0");
     cudaStream_t st = (cudaStream_t)stream;
     // few rows (M <= 128) and not enough 128-wide tiles to occupy every SM twice: 32-wide tiles (weight streaming)
     if (M <= BM && !b_mn && (long long)((N + 127) / 128) < 2LL * sm_count() && N % 32 == 0)
