@@ -176,6 +176,36 @@ size_t tl_sample_ws(int M);
 int tl_sample(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
               unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream);
 
+/* ---- logits processors (csrc/logits_process.cu): HF's RepetitionPenaltyLogitsProcessor -> NoRepeatNGramLogitsProcessor
+ * -> MinNewTokensLengthLogitsProcessor on the fp32 copy of the bf16 logits, before the argmax or the warpers above.
+ * Each row keeps its token history in device memory: log int32[M, L] (row pitch L), len int32[M] and a presence
+ * bitmap bits uint32[M, ceil(V/32)].  params_dev int32[TL_LP_PARAMS]: the penalty (float bits), n, min_new_tokens,
+ * the prompt length (history entries that are not generated), the number of EOS ids and the ids.  The picking kernel
+ * appends its id to the row's history, so a captured graph stays right on every replay.
+ * flags & TL_LP_BAN: compute the ban set (n-gram completions, EOS ids below min_new_tokens); otherwise only the
+ * penalty applies.  workspace >= tl_logits_proc_ws(M, V) bytes. */
+#define TL_LP_PENALTY 0
+#define TL_LP_NGRAM 1
+#define TL_LP_MIN_NEW 2
+#define TL_LP_PROMPT 3
+#define TL_LP_N_EOS 4
+#define TL_LP_EOS 5
+#define TL_LP_MAX_EOS 8
+#define TL_LP_PARAMS (TL_LP_EOS + TL_LP_MAX_EOS)
+#define TL_LP_BAN 1
+size_t tl_logits_proc_ws(int M, int V);
+/* history of row m = prompt[m, 0:S] (int64 [M,S]); len = S; the bitmap holds exactly those ids */
+int tl_history_fill(const int64_t* prompt, int32_t* log, int32_t* len, uint32_t* bits, int M, int S, int L, int V,
+                    void* stream);
+/* ids[m] = the lowest index of the largest processed value (torch.argmax); 0 when every value is -inf */
+int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                   const int32_t* params_dev, int flags, void* workspace, size_t ws_bytes, int M, int V, int L, void* stream);
+/* tl_sample's rules over the processed values (32-bit keys: the top-k and top-p boundaries are resolved exactly, and the
+ * probability mass is summed as 64-bit fixed-point integers, so a seed reproduces its tokens) */
+int tl_sample_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                   const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
+                   unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream);
+
 /* ---- small device-side helpers used by the captured decode graph */
 int tl_advance_pos(int32_t* pos_dev, int32_t* kv_len_dev, int delta, void* stream); /* pos += delta; kv_len = pos */
 /* out_tokens[b, *step_dev] = ids[b] for b < B (row pitch ld), then ++*step_dev: the generated-token log

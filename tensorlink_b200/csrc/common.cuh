@@ -60,6 +60,35 @@ __device__ __forceinline__ float warp_max(float v) {
     return v;
 }
 
+// ---------------------------------------------------------------- logits processors (csrc/logits_process.cu)
+// One row's token history (log, length, presence bitmap) and the parameters, as tl_argmax_proc / tl_sample_proc get them.
+struct LpRows {
+    int32_t* log;               // [M, L]
+    int32_t* len;               // [M]
+    uint32_t* bits;             // [M, W]: bit v set = token v is in the history
+    const uint32_t* ban;        // [M, W] ban set of this step, or nullptr
+    const int32_t* params;      // TL_LP_* layout (include/tensorlink_b200.h)
+    int L, W;
+};
+__host__ __device__ __forceinline__ int lp_words(int V) { return (V + 31) / 32; }
+inline size_t lp_ban_bytes(int M, int V) { return ((size_t)M * lp_words(V) * sizeof(uint32_t) + 255) & ~(size_t)255; }
+// HF RepetitionPenaltyLogitsProcessor on the fp32 copy of a logit, then the ban set (-inf)
+__device__ __forceinline__ float lp_value(float s, int i, const uint32_t* bits, const uint32_t* ban, float penalty) {
+    if (ban && ((ban[i >> 5] >> (i & 31)) & 1u)) return -INFINITY;
+    if ((bits[i >> 5] >> (i & 31)) & 1u) s = s < 0.f ? __fmul_rn(s, penalty) : __fdiv_rn(s, penalty);
+    return s;
+}
+// the picked token joins row m's history (one thread per row)
+__device__ __forceinline__ void lp_append(const LpRows& h, int m, int id) {
+    const int n = h.len[m];
+    if (n < h.L) h.log[(size_t)m * h.L + n] = id;
+    h.len[m] = n + 1;
+    h.bits[(size_t)m * h.W + (id >> 5)] |= 1u << (id & 31);
+}
+// the ban set of every row into h.ban (the first lp_ban_bytes(M, V) of the workspace): n-gram completions and the EOS
+// ids while below min_new_tokens
+int lp_ban_launch(const LpRows& h, uint32_t* ban, int M, int V, cudaStream_t stream);
+
 // ---------------------------------------------------------------- mbarrier / TMA PTX
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));

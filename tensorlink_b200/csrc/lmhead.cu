@@ -1,22 +1,29 @@
 // Final RMSNorm + lm_head + greedy argmax for decode-shaped inputs (M <= 8 rows).
 // logits are produced by the weight-streaming GEMV (bf16, as the reference's lm_head emits them), then a
 // two-stage argmax picks the lowest index among equal maxima, which is what torch.argmax returns.
+// With PROC the argmax runs over HF's processed values (repetition penalty, ban set: logits_process.cu), computed in
+// fp32 as each logit is read, and the final stage appends the picked id to the row's history.
 #include "common.cuh"
 
 namespace tl {
 
 constexpr int AM_PARTS = 64, AM_THREADS = 256;
 
+template <bool PROC>
 __global__ void __launch_bounds__(AM_THREADS) argmax_part_kernel(const bf16* __restrict__ logits, float* __restrict__ pval,
-                                                                 int* __restrict__ pidx, int V) {
+                                                                 int* __restrict__ pidx, int V, LpRows h) {
     const int m = blockIdx.y, part = blockIdx.x;
     const int per = (V + AM_PARTS - 1) / AM_PARTS;
     const int lo = part * per, hi = min(V, lo + per);
     const bf16* row = logits + (size_t)m * V;
+    const uint32_t* bits = PROC ? h.bits + (size_t)m * h.W : nullptr;
+    const uint32_t* ban = PROC && h.ban ? h.ban + (size_t)m * h.W : nullptr;
+    const float penalty = PROC ? __int_as_float(h.params[TL_LP_PENALTY]) : 1.f;
     float best = -INFINITY;
     int bi = 0x7fffffff;
     for (int i = lo + threadIdx.x; i < hi; i += AM_THREADS) {
-        const float v = bf2f(row[i]);
+        float v = bf2f(row[i]);
+        if (PROC) v = lp_value(v, i, bits, ban, penalty);
         if (v > best) { best = v; bi = i; }     // ascending i per thread: first max kept
     }
 #pragma unroll
@@ -37,8 +44,9 @@ __global__ void __launch_bounds__(AM_THREADS) argmax_part_kernel(const bf16* __r
     }
 }
 
+template <bool PROC>
 __global__ void argmax_final_kernel(const float* __restrict__ pval, const int* __restrict__ pidx,
-                                    int64_t* __restrict__ ids_out) {
+                                    int64_t* __restrict__ ids_out, LpRows h) {
     const int m = blockIdx.x, lane = threadIdx.x;
     float best = -INFINITY;
     int bi = 0x7fffffff;
@@ -53,7 +61,11 @@ __global__ void argmax_final_kernel(const float* __restrict__ pval, const int* _
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
         if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
     }
-    if (lane == 0) ids_out[m] = (bi == 0x7fffffff) ? 0 : (int64_t)bi;
+    if (lane == 0) {
+        const int id = (bi == 0x7fffffff) ? 0 : bi;
+        ids_out[m] = (int64_t)id;
+        if (PROC) lp_append(h, m, id);
+    }
 }
 
 }  // namespace tl
@@ -72,9 +84,30 @@ int tl_argmax_bf16(const void* logits, int64_t* ids_out, void* workspace, size_t
     float* pval = (float*)workspace;
     int* pidx = (int*)(pval + (size_t)M * AM_PARTS);
     cudaStream_t st = (cudaStream_t)stream;
-    argmax_part_kernel<<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V);
-    argmax_final_kernel<<<M, 32, 0, st>>>(pval, pidx, ids_out);
+    argmax_part_kernel<false><<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V, LpRows{});
+    argmax_final_kernel<false><<<M, 32, 0, st>>>(pval, pidx, ids_out, LpRows{});
     return check_launch("tl_argmax_bf16");
+}
+
+int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                   const int32_t* params_dev, int flags, void* workspace, size_t ws_bytes, int M, int V, int L, void* stream) {
+    using namespace tl;
+    TL_REQUIRE(logits && ids_out && log && len && bits && params_dev && workspace, TL_ERR_INVALID, "tl_argmax_proc: null argument");
+    TL_REQUIRE(M >= 1 && V >= 1 && L >= 1, TL_ERR_INVALID, "tl_argmax_proc: bad shape M=%d V=%d L=%d", M, V, L);
+    TL_REQUIRE(ws_bytes >= tl_logits_proc_ws(M, V), TL_ERR_WORKSPACE, "tl_argmax_proc: workspace %zu < %zu", ws_bytes,
+               tl_logits_proc_ws(M, V));
+    cudaStream_t st = (cudaStream_t)stream;
+    uint32_t* ban = (uint32_t*)workspace;
+    float* pval = (float*)((unsigned char*)workspace + lp_ban_bytes(M, V));
+    int* pidx = (int*)(pval + (size_t)M * AM_PARTS);
+    const LpRows h{log, len, bits, (flags & TL_LP_BAN) ? ban : nullptr, params_dev, L, lp_words(V)};
+    if (flags & TL_LP_BAN) {
+        const int rc = lp_ban_launch(h, ban, M, V, st);
+        if (rc != TL_OK) return rc;
+    }
+    argmax_part_kernel<true><<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V, h);
+    argmax_final_kernel<true><<<M, 32, 0, st>>>(pval, pidx, ids_out, h);
+    return check_launch("tl_argmax_proc");
 }
 
 int tl_lmhead_argmax(const void* x, const void* W, const void* norm_w, float eps, int64_t* ids_out, void* logits_out,

@@ -189,9 +189,207 @@ __global__ void __launch_bounds__(SM_THREADS) sample_kernel(const bf16* __restri
     }
 }
 
+// ================================================================================================ processed sampling
+// After the logits processors (logits_process.cu) a value is an arbitrary fp32, no longer one of 65536 bf16 patterns, so
+// the rules above run on 32-bit monotone keys: a histogram of the high 16 key bits finds the boundary bin, and a second
+// pass over the elements of that bin finds the boundary key.  Probability mass is summed as 64-bit fixed-point integers
+// (2^40 = the row's maximum), so every sum is exact and independent of the order the atomics land in.
+typedef unsigned long long u64;
+constexpr double SP_ONE = 1099511627776.0;       // 2^40
+
+__device__ __forceinline__ uint32_t f32_key(float v) {     // monotone; -0 and +0 share the key of +0
+    const uint32_t b = __float_as_uint(v == 0.f ? 0.f : v);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float key_f32(uint32_t k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+__device__ __forceinline__ u64 key_weight(uint32_t key, float inv_temp, float x_max) {
+    return (u64)((double)expf(key_f32(key) * inv_temp - x_max) * SP_ONE);
+}
+
+__device__ u64 block_excl_scan_u64(u64 v, u64* s_warp, u64* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    u64 x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const u64 y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        u64 w = s_warp[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const u64 y = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w += y;
+        }
+        s_warp[lane] = w;
+    }
+    __syncthreads();
+    const u64 before = (warp ? s_warp[warp - 1] : 0ull) + (x - v);
+    *total = s_warp[31];
+    __syncthreads();
+    return before;
+}
+
+struct Crossing { int bin; u64 above, T; };
+
+// Walking the 65536 bins of h downwards: the bin b with above(b) < T <= above(b) + h[b], where above(b) is the sum of the
+// bins over b and T = T_abs, or ceil(frac * total) when frac >= 0.  All comparisons are integer: exactly one bin.
+__device__ Crossing find_crossing(const u64* h, u64 T_abs, float frac, u64* s_warp, Crossing* s_out) {
+    const int hi = SM_BINS - 1 - (int)threadIdx.x * SM_PER;
+    u64 local = 0;
+    for (int j = 0; j < SM_PER; ++j) local += h[hi - j];
+    u64 total;
+    const u64 before = block_excl_scan_u64(local, s_warp, &total);
+    const u64 T = frac < 0.f ? T_abs : (u64)ceil((double)frac * (double)total);
+    if (before < T && T <= before + local) {
+        u64 c = before;
+        for (int j = 0; j < SM_PER; ++j) {
+            const u64 x = h[hi - j];
+            if (c + x >= T) { *s_out = Crossing{hi - j, c, T}; break; }
+            c += x;
+        }
+    }
+    __syncthreads();
+    const Crossing r = *s_out;
+    __syncthreads();
+    return r;
+}
+
+__device__ __forceinline__ void clear_bins(u64* h) {
+    for (int i = threadIdx.x; i < SM_BINS; i += SM_THREADS) h[i] = 0ull;
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(SM_THREADS) sample_proc_kernel(const bf16* __restrict__ logits, int64_t* __restrict__ ids_out,
+                                                                 int V, LpRows h, float inv_temp, int top_k, float top_p,
+                                                                 unsigned long long seed, int32_t* __restrict__ counters,
+                                                                 u64* __restrict__ hist_all) {
+    const int row = blockIdx.x, tid = threadIdx.x;
+    const bf16* lr = logits + (size_t)row * V;
+    const uint32_t* bits = h.bits + (size_t)row * h.W;
+    const uint32_t* ban = h.ban ? h.ban + (size_t)row * h.W : nullptr;
+    const float penalty = __int_as_float(h.params[TL_LP_PENALTY]);
+    u64* hist = hist_all + (size_t)row * SM_BINS;
+    __shared__ u64 s_warp[32];
+    __shared__ float s_max[32];
+    __shared__ Crossing s_cross;
+    __shared__ int s_pick;
+    auto key_at = [&](int i) { return f32_key(lp_value(bf2f(lr[i]), i, bits, ban, penalty)); };
+    const bool use_k = top_k > 0 && top_k < V;
+    // ---- max (and the top-k count histogram of the high key bits)
+    if (use_k) clear_bins(hist);
+    float vmax = -INFINITY;
+    for (int i = tid; i < V; i += SM_THREADS) {
+        const uint32_t key = key_at(i);
+        vmax = fmaxf(vmax, key_f32(key));
+        if (use_k) atomicAdd(&hist[key >> 16], 1ull);
+    }
+    vmax = warp_max(vmax);
+    if ((tid & 31) == 0) s_max[tid >> 5] = vmax;
+    __syncthreads();
+    vmax = warp_max(s_max[tid & 31]);
+    const uint32_t ctr = (uint32_t)counters[row];
+    if (vmax == -INFINITY) {                  // every token banned: token 0, as the argmax returns
+        if (tid == 0) {
+            ids_out[row] = 0;
+            counters[row] = (int32_t)(ctr + 1u);
+            lp_append(h, row, 0);
+        }
+        return;
+    }
+    const float x_max = vmax * inv_temp;
+    // ---- top-k: the key of the k-th largest value; every value >= it is kept
+    uint32_t k_key = 0;
+    if (use_k) {
+        const Crossing c = find_crossing(hist, (u64)top_k, -1.f, s_warp, &s_cross);
+        clear_bins(hist);
+        for (int i = tid; i < V; i += SM_THREADS) {
+            const uint32_t key = key_at(i);
+            if ((int)(key >> 16) == c.bin) atomicAdd(&hist[key & 0xffffu], 1ull);
+        }
+        __syncthreads();
+        const Crossing lo = find_crossing(hist, c.T - c.above, -1.f, s_warp, &s_cross);
+        k_key = ((uint32_t)c.bin << 16) | (uint32_t)lo.bin;
+    }
+    // ---- top-p: the lowest key whose mass above is < top_p * Z (its whole tie group is kept)
+    uint32_t p_key = k_key;
+    if (top_p < 1.0f) {
+        clear_bins(hist);
+        for (int i = tid; i < V; i += SM_THREADS) {
+            const uint32_t key = key_at(i);
+            if (key >= k_key) atomicAdd(&hist[key >> 16], key_weight(key, inv_temp, x_max));
+        }
+        __syncthreads();
+        const Crossing c = find_crossing(hist, 0ull, top_p, s_warp, &s_cross);
+        clear_bins(hist);
+        for (int i = tid; i < V; i += SM_THREADS) {
+            const uint32_t key = key_at(i);
+            if (key >= k_key && (int)(key >> 16) == c.bin) atomicAdd(&hist[key & 0xffffu], key_weight(key, inv_temp, x_max));
+        }
+        __syncthreads();
+        const Crossing lo = find_crossing(hist, c.T - c.above, -1.f, s_warp, &s_cross);
+        p_key = ((uint32_t)c.bin << 16) | (uint32_t)lo.bin;
+    }
+    // ---- draw and invert the CDF over the kept tokens in index order (integer prefix sums: exact)
+    const int per = (V + SM_THREADS - 1) / SM_THREADS;
+    const int i0 = tid * per, i1 = min(V, i0 + per);
+    u64 local_w = 0;
+    for (int i = i0; i < i1; ++i) {
+        const uint32_t key = key_at(i);
+        if (key >= p_key) local_w += key_weight(key, inv_temp, x_max);
+    }
+    if (tid == 0) s_pick = -1;
+    u64 W;
+    const u64 w_before = block_excl_scan_u64(local_w, s_warp, &W);
+    const u64 target = min(W - 1, (u64)((double)philox_uniform(seed, (uint32_t)row, ctr) * (double)W));
+    if (local_w > 0 && w_before <= target && target < w_before + local_w) {
+        u64 c = w_before;
+        for (int i = i0; i < i1; ++i) {
+            const uint32_t key = key_at(i);
+            if (key < p_key) continue;
+            c += key_weight(key, inv_temp, x_max);
+            if (target < c) { s_pick = i; break; }
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        const int pick = s_pick < 0 ? 0 : s_pick;
+        ids_out[row] = (int64_t)pick;
+        counters[row] = (int32_t)(ctr + 1u);
+        lp_append(h, row, pick);
+    }
+}
+
 }  // namespace tl
 
 extern "C" {
+
+int tl_sample_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                   const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
+                   unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream) {
+    using namespace tl;
+    TL_REQUIRE(logits && ids_out && log && len && bits && params_dev && counters_dev && workspace, TL_ERR_INVALID,
+               "tl_sample_proc: null argument");
+    TL_REQUIRE(M >= 1 && V >= 1 && L >= 1, TL_ERR_INVALID, "tl_sample_proc: bad shape M=%d V=%d L=%d", M, V, L);
+    TL_REQUIRE(temperature > 0.f && top_p > 0.f && top_p <= 1.f && top_k >= 0, TL_ERR_INVALID,
+               "tl_sample_proc: temperature must be > 0, 0 < top_p <= 1, top_k >= 0 (got %g, %g, %d)", temperature, top_p, top_k);
+    TL_REQUIRE(ws_bytes >= tl_logits_proc_ws(M, V), TL_ERR_WORKSPACE, "tl_sample_proc: workspace %zu < %zu", ws_bytes,
+               tl_logits_proc_ws(M, V));
+    cudaStream_t st = (cudaStream_t)stream;
+    uint32_t* ban = (uint32_t*)workspace;
+    const LpRows h{log, len, bits, (flags & TL_LP_BAN) ? ban : nullptr, params_dev, L, lp_words(V)};
+    if (flags & TL_LP_BAN) {
+        const int rc = lp_ban_launch(h, ban, M, V, st);
+        if (rc != TL_OK) return rc;
+    }
+    sample_proc_kernel<<<M, SM_THREADS, 0, st>>>((const bf16*)logits, ids_out, V, h, 1.0f / temperature, top_k, top_p, seed,
+                                                 counters_dev, (u64*)((unsigned char*)workspace + lp_ban_bytes(M, V)));
+    return check_launch("tl_sample_proc");
+}
 
 size_t tl_sample_ws(int M) { return (size_t)(M > 0 ? M : 0) * tl::SM_BINS * sizeof(uint32_t); }
 

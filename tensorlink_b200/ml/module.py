@@ -13,6 +13,7 @@ the last stage (pass ``gather_logits=True`` to copy them to rank 0).
 """
 from __future__ import annotations
 
+import numbers
 import os
 
 import time
@@ -21,6 +22,7 @@ from typing import Any, Callable, Dict, Optional, Union
 
 import torch
 
+from ..native import LP_MAX_EOS
 from ..p2p.link import StageLink, init_process_group_from_env
 from . import graphing
 from .configs import ShardModelConfig, get_config
@@ -68,6 +70,27 @@ def _check_unconsumed(kwargs: dict, what: str):
         if ok is None or not any(v is o or (o is not None and v == o) for o in ok):
             raise NotImplementedError(f"{what}: keyword {k}={v!r} is not supported by the H100 stage executor "
                                       "(it would be silently ignored otherwise)")
+
+
+def _logits_processors(repetition_penalty=None, no_repeat_ngram_size=None, min_new_tokens=None,
+                       eos_token_id=None) -> Optional[dict]:
+    """HF's ``repetition_penalty`` / ``no_repeat_ngram_size`` / ``min_new_tokens`` as {penalty, ngram, min_new, eos}, or
+    None when every one is at its neutral value (1.0 / 0 / 0, or None).  ``eos`` lists the EOS ids ``min_new_tokens``
+    holds back (empty without it or without ``eos_token_id``, where HF's processor is a no-op).  Invalid values raise
+    ValueError, as HF does; more EOS ids than the device parameter block holds raise NotImplementedError."""
+    p = 1.0 if repetition_penalty is None else repetition_penalty
+    if isinstance(p, bool) or not isinstance(p, numbers.Real) or not p > 0:
+        raise ValueError(f"repetition_penalty has to be a strictly positive float, but is {repetition_penalty!r}")
+    n, k = (0 if v is None else v for v in (no_repeat_ngram_size, min_new_tokens))
+    for name, v in (("no_repeat_ngram_size", n), ("min_new_tokens", k)):
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral) or v < 0:
+            raise ValueError(f"{name} has to be a non-negative integer, but is {v!r}")
+    if p == 1.0 and n == 0 and k == 0:
+        return None
+    eos = _eos_list(eos_token_id) if k > 0 else []
+    if len(eos) > LP_MAX_EOS:
+        raise NotImplementedError(f"min_new_tokens with {len(eos)} EOS ids (at most {LP_MAX_EOS})")
+    return {"penalty": float(p), "ngram": int(n), "min_new": int(k), "eos": eos}
 
 
 def _check_attention_mask(mask, shape):
@@ -457,6 +480,9 @@ class DistributedModel(torch.nn.Module):
         token on the last stage's GPU from the distribution HF's warpers define — ``temperature`` (default 1.0), ``top_k``
         (default 50, 0 = off), ``top_p`` (default 1.0) — with a counter-based Philox stream keyed by ``seed`` (extension;
         default ``torch.initial_seed()``): the same seed reproduces the same tokens (csrc/sample.cu).
+        ``repetition_penalty``, ``no_repeat_ngram_size`` and ``min_new_tokens`` act as HF's logits processors, in that
+        order and before the sampling warpers, on the last stage's GPU inside the decode graph (csrc/logits_process.cu).
+        As in HF the history they look at is the whole ``input_ids`` row, pad tokens included, plus the generated tokens.
         ``input_ids`` [B,S] int64 on the first stage; returns [B,S+new] on every rank.
         ``streamer``: object with ``put(tensor)`` / ``end()`` (HF BaseStreamer protocol), called on rank 0
         with each new token column, all batch rows (the reference streams row 0 only, worker.py:134-139).
@@ -479,6 +505,8 @@ class DistributedModel(torch.nn.Module):
             if sampling["temperature"] <= 0 or not (0 < sampling["top_p"] <= 1) or sampling["top_k"] < 0:
                 raise ValueError(f"invalid sampling parameters {sampling}")
         self._eos = (kwargs.pop("eos_token_id", None), kwargs.pop("pad_token_id", None))
+        procs = _logits_processors(kwargs.pop("repetition_penalty", None), kwargs.pop("no_repeat_ngram_size", None),
+                                   kwargs.pop("min_new_tokens", None), self._eos[0])
         mask = kwargs.pop("attention_mask", None)
         _check_unconsumed(kwargs, "DistributedModel.generate")
         link, st, cfg = self.link, self.stage, self.cfg
@@ -496,20 +524,30 @@ class DistributedModel(torch.nn.Module):
                 g = _left_pad_groups(mask)
                 groups = None if g is None else (g, tuple(input_ids.shape))
         if self.world > 1:
-            groups, padded = link.broadcast_object((groups, padded))
+            groups, padded, procs = link.broadcast_object((groups, padded, procs))
+        if procs is not None and not hasattr(st, "set_logits_processors"):
+            raise NotImplementedError("repetition_penalty / no_repeat_ngram_size / min_new_tokens need the CUDA stage")
         if groups is not None:
+            if procs is not None:                # the grouped runs would see each row's history without its pads
+                raise NotImplementedError("repetition_penalty / no_repeat_ngram_size / min_new_tokens with a left-padded "
+                                          "batch need a stage with per-row key starts (supports_kv_start)")
             return self._generate_left_padded(input_ids, groups[0], groups[1], max_new, streamer, use_graph, sampling)
-        result = self._generate_batch(input_ids, max_new, streamer, use_graph, profile, sampling,
+        if procs is not None and link.first:     # the starting history: every column, the dropped pad columns too
+            procs["history"] = input_ids.cpu() if padded is None else torch.cat([padded[0], input_ids.cpu()], dim=1)
+        result = self._generate_batch(input_ids, max_new, streamer, use_graph, profile, sampling, procs,
                                       None if padded is None else padded[1])
         if padded is not None and padded[0].shape[1]:
             result = torch.cat([padded[0].to(result.device), result], dim=1)
         return result
 
-    def _generate_batch(self, input_ids, max_new, streamer, use_graph, profile, sampling, kv_start):
-        """One run of the batch: prefill every micro-batch, then the decode loop.  ``kv_start``: the per-row key starts
-        of a left-padded batch, or None."""
+    def _generate_batch(self, input_ids, max_new, streamer, use_graph, profile, sampling, procs, kv_start):
+        """One run of the batch: prefill every micro-batch, then the decode loop.  ``procs``: the logits processors
+        (``_logits_processors``) or None; on the first stage ``procs["history"]`` holds their starting history [B, S']
+        (``input_ids`` plus any pad columns dropped before the run), which the first stage sends to the last one here,
+        once.  ``kv_start``: the per-row key starts of a left-padded batch, or None."""
         link, st, cfg = self.link, self.stage, self.cfg
-        shape, sampling = link.broadcast_object((tuple(input_ids.shape), sampling) if link.first else None)
+        shape, sampling, procs = link.broadcast_object((tuple(input_ids.shape), sampling, procs) if link.first else None)
+        prompt = None if procs is None else procs.pop("history")
         B, S = shape
         if hasattr(st, "set_sampling"):
             st.set_sampling(sampling)               # the last stage draws; greedy (None) restores the argmax path
@@ -517,6 +555,11 @@ class DistributedModel(torch.nn.Module):
                 st.sample_ctr.zero_()               # a seed names ONE stream: the same call reproduces its tokens
         elif sampling is not None:
             raise NotImplementedError("sampling needs the CUDA stage")
+        if hasattr(st, "set_logits_processors"):
+            st.set_logits_processors(None if procs is None else dict(procs, prompt_len=prompt.shape[1]),
+                                     0 if procs is None else prompt.shape[1] + max_new)
+        elif procs is not None:
+            raise NotImplementedError("repetition_penalty / no_repeat_ngram_size / min_new_tokens need the CUDA stage")
         n_mb = min(self.n_pipelines, B)
         while B % n_mb:                      # the largest micro-batch count <= n_pipelines that divides the batch
             n_mb -= 1
@@ -535,6 +578,9 @@ class DistributedModel(torch.nn.Module):
             for g in st.slots:                       # NCCL kernels share the SMs during decode: no persistent all-SM kernel
                 if hasattr(g, "allow_chain"):
                     g.allow_chain = False
+        if procs is not None and st.has_head:
+            for m in range(n_mb):
+                st.fill_history(m, prompt[m * b:(m + 1) * b].to(dev))
         if ring is not None:
             if max_new > ring.max_new:
                 raise ValueError(f"max_new_tokens {max_new} exceeds the token log of the peer ring ({ring.max_new})")

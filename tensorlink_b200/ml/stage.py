@@ -50,6 +50,12 @@ class CudaStage:
             self.sampling: Optional[dict] = None        # set by generate(do_sample=True): temperature / top_k / top_p / seed
             self.sample_ctr = torch.zeros(n_slots, max_batch, dtype=torch.int32, device=dev)
             self.sample_ws: Optional[torch.Tensor] = None
+            # logits processors (set_logits_processors): per slot and row a token history on the device -- log
+            # [n_slots, max_batch, L], length, presence bitmap of V bits -- and the parameters (penalty, n, ...)
+            self.procs: Optional[dict] = None
+            self.lp_flags = 0
+            self.hist_log: Optional[torch.Tensor] = None
+            self.hist_len = self.hist_bits = self.lp_params = self.lp_ws = None
 
     # ------------------------------------------------------------------------------------------ pieces
     def embed(self, ids: torch.Tensor) -> torch.Tensor:
@@ -79,15 +85,65 @@ class CudaStage:
         if sampling is not None and self.sample_ws is None:
             self.sample_ws = torch.empty(nat.sample_ws(self.max_batch), dtype=torch.uint8, device=self.device)
 
+    def set_logits_processors(self, procs: Optional[dict], length: int = 0):
+        """HF's repetition penalty / no-repeat n-gram / min-new-tokens on the last stage; None = off.  ``procs``: penalty,
+        ngram, min_new, eos (ids), prompt_len (history entries that are prompt); ``length``: the longest history of the
+        run (prompt width + max_new_tokens).  Switching on or off, or the ban set on or off, drops the captured decode
+        graphs (the launch sequence differs); the values live in device memory, so changing them keeps the graphs."""
+        if not self.has_head:
+            return
+        flags = 0 if procs is None else (nat.LP_BAN if procs["ngram"] > 0 or (procs["min_new"] > 0 and procs["eos"]) else 0)
+        if (procs is None) != (self.procs is None) or flags != self.lp_flags:
+            self.graphs.clear()
+        self.procs, self.lp_flags = procs, flags
+        if procs is None:
+            return
+        n_slots, dev, V = len(self.slots), self.device, self.cfg.vocab
+        if self.lp_ws is None:
+            self.lp_ws = torch.empty(nat.logits_proc_ws(self.max_batch, V), dtype=torch.uint8, device=dev)
+            self.lp_params = torch.zeros(nat.LP_PARAMS, dtype=torch.int32, device=dev)
+            self.hist_len = torch.zeros(n_slots, self.max_batch, dtype=torch.int32, device=dev)
+            self.hist_bits = torch.zeros(n_slots, self.max_batch, (V + 31) // 32, dtype=torch.int32, device=dev)
+        if self.hist_log is None or self.hist_log.shape[2] < length:
+            self.hist_log = torch.zeros(n_slots, self.max_batch, max(length, self.max_seq), dtype=torch.int32, device=dev)
+            self.graphs.clear()                      # the captured kernels hold the old log's address
+        self.lp_params.copy_(nat.lp_params(procs["penalty"], procs["ngram"], procs["min_new"], procs["prompt_len"],
+                                           procs["eos"] if procs["min_new"] > 0 else []))
+
+    def fill_history(self, slot: int, prompt: torch.Tensor):
+        """Row r of ``slot`` starts its token history with ``prompt[r]`` (int64 [b, S] on this device, pad columns included)."""
+        nat.history_fill(prompt.contiguous(), self.hist_log[slot], self.hist_len[slot], self.hist_bits[slot], self.cfg.vocab)
+
     def head_argmax(self, hidden: torch.Tensor, ids_out: torch.Tensor, slot: int = 0):
         """next token for [B,H] rows -> ids_out [B] int64: greedy (bit-exact target: torch.argmax of bf16 logits) or, after
-        ``set_sampling``, one draw per row from the warped distribution (csrc/sample.cu)."""
+        ``set_sampling``, one draw per row from the warped distribution (csrc/sample.cu).  With logits processors on, both
+        act on HF's processed scores and append the picked id to the row's history."""
+        if self.procs is not None:
+            self._head_processed(hidden, ids_out, slot)
+            return
         self._head_greedy(hidden, ids_out)
         if self.sampling is not None:
             B = hidden.shape[0]
             s = self.sampling
             nat.sample(self.logits_dec[:B], ids_out, self.sample_ctr[slot], self.sample_ws, s["temperature"], s["top_k"], s["top_p"],
                        s["seed"] + 0x9E3779B97F4A7C15 * slot)
+
+    def _head_processed(self, hidden: torch.Tensor, ids_out: torch.Tensor, slot: int):
+        cfg, v = self.cfg, self.params.v
+        B = hidden.shape[0]
+        logits = self.logits_dec[:B]
+        if B <= gemv_max_rows():
+            nat.gemv(hidden, v["head"], out=logits, norm_w=v["norm"], eps=cfg.rms_eps)     # the logits tl_lmhead_argmax makes
+        else:
+            nat.rmsnorm_fwd(hidden, v["norm"], cfg.rms_eps, out=self.hn[:B])
+            nat.gemm(self.hn[:B], v["head"], out=logits)
+        hist = (self.hist_log[slot], self.hist_len[slot], self.hist_bits[slot], self.lp_params)
+        if self.sampling is None:
+            nat.argmax_proc(logits, ids_out, *hist, self.lp_ws, self.lp_flags)
+        else:
+            s = self.sampling
+            nat.sample_proc(logits, ids_out, *hist, self.sample_ctr[slot], self.lp_ws, s["temperature"], s["top_k"], s["top_p"],
+                            s["seed"] + 0x9E3779B97F4A7C15 * slot, self.lp_flags)
 
     def _head_greedy(self, hidden: torch.Tensor, ids_out: torch.Tensor):
         cfg, v = self.cfg, self.params.v
@@ -145,6 +201,9 @@ class CudaStage:
             grp = self.slots[slot]
             saved = (grp.pos_dev.clone(), grp.kvlen_dev.clone(), self.ids_dec[slot].clone(), self.x_dec[slot].clone())
             ctr_saved = self.sample_ctr.clone() if self.has_head else None      # the warm-up step must not consume a draw
+            hist_saved = None                                                   # ... nor join a row's token history
+            if self.has_head and self.procs is not None:
+                hist_saved = (self.hist_len.clone(), self.hist_bits.clone())
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
@@ -154,6 +213,8 @@ class CudaStage:
             self.ids_dec[slot].copy_(saved[2]); self.x_dec[slot].copy_(saved[3])
             if ctr_saved is not None:
                 self.sample_ctr.copy_(ctr_saved)
+            if hist_saved is not None:
+                self.hist_len.copy_(hist_saved[0]); self.hist_bits.copy_(hist_saved[1])
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):

@@ -73,6 +73,11 @@ _SIGS = {
     "tl_sample_ws": (c_size_t, [c_int]),
     "tl_sample": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p, c_void_p, c_size_t,
                           c_void_p]),
+    "tl_logits_proc_ws": (c_size_t, [c_int, c_int]),
+    "tl_history_fill": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "tl_argmax_proc": (c_int, [c_void_p] * 6 + [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
+    "tl_sample_proc": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p,
+                                                c_void_p, c_size_t, c_void_p]),
     "tl_advance_pos": (c_int, [c_void_p, c_void_p, c_int, c_void_p]),
     "tl_append_token": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "tl_swiglu_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
@@ -383,6 +388,71 @@ def sample(logits, ids_out, counters, ws, temperature: float = 1.0, top_k: int =
     assert ids_out.dtype == torch.int64 and counters.dtype == torch.int32 and counters.numel() >= M
     _check(load().tl_sample(_p(logits), _p(ids_out), M, V, float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1),
                             _p(counters), _p(ws), ws.numel() * ws.element_size(), _stream()), "tl_sample")
+
+
+LP_PENALTY, LP_NGRAM, LP_MIN_NEW, LP_PROMPT, LP_N_EOS, LP_EOS, LP_MAX_EOS = 0, 1, 2, 3, 4, 5, 8
+LP_PARAMS = LP_EOS + LP_MAX_EOS
+LP_BAN = 1
+
+
+def logits_proc_ws(M: int, V: int) -> int:
+    return int(load().tl_logits_proc_ws(M, V))
+
+
+def _history(log, length, bits, M: int, V: int):
+    """A token history (include/tensorlink_b200.h, logits processors): log int32 [>=M, L], len int32 [>=M], bits int32
+    [>=M, ceil(V/32)] (the bitmap's words; torch has no uint32), all contiguous on the device."""
+    for t in (log, length, bits):
+        if t.dtype != torch.int32 or not t.is_cuda or not t.is_contiguous() or t.shape[0] < M:
+            raise NativeError(f"history tensors must be contiguous int32 CUDA tensors of at least {M} rows")
+    if bits.shape[1] != (V + 31) // 32:
+        raise NativeError(f"history bitmap has {bits.shape[1]} words per row, V={V} needs {(V + 31) // 32}")
+    return log.shape[1]
+
+
+def history_fill(prompt, log, length, bits, V: int):
+    """The history of row m becomes prompt[m] (int64 [M,S]): log[m, :S], len[m] = S and the presence bitmap."""
+    require_device()
+    assert prompt.dtype == torch.int64 and prompt.is_contiguous()
+    M, S = prompt.shape
+    L = _history(log, length, bits, M, V)
+    _check(load().tl_history_fill(_p(prompt), _p(log), _p(length), _p(bits), M, S, L, V, _stream()), "tl_history_fill")
+
+
+def argmax_proc(logits, ids_out, log, length, bits, params, ws, flags: int = 0):
+    """ids_out[m] = torch.argmax of HF's processed fp32 scores of logits[m]; appends the id to row m's history."""
+    require_device()
+    _bf16(logits)
+    M, V = logits.shape
+    L = _history(log, length, bits, M, V)
+    assert ids_out.dtype == torch.int64 and params.dtype == torch.int32 and params.numel() >= LP_PARAMS
+    _check(load().tl_argmax_proc(_p(logits), _p(ids_out), _p(log), _p(length), _p(bits), _p(params), flags, _p(ws),
+                                 ws.numel() * ws.element_size(), M, V, L, _stream()), "tl_argmax_proc")
+
+
+def sample_proc(logits, ids_out, log, length, bits, params, counters, ws, temperature: float = 1.0, top_k: int = 0,
+                top_p: float = 1.0, seed: int = 0, flags: int = 0):
+    """``sample`` over HF's processed fp32 scores; appends the drawn id to row m's history."""
+    require_device()
+    _bf16(logits)
+    M, V = logits.shape
+    L = _history(log, length, bits, M, V)
+    assert ids_out.dtype == torch.int64 and counters.dtype == torch.int32 and counters.numel() >= M
+    assert params.dtype == torch.int32 and params.numel() >= LP_PARAMS
+    _check(load().tl_sample_proc(_p(logits), _p(ids_out), _p(log), _p(length), _p(bits), _p(params), flags, M, V, L,
+                                 float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1), _p(counters),
+                                 _p(ws), ws.numel() * ws.element_size(), _stream()), "tl_sample_proc")
+
+
+def lp_params(penalty: float, ngram: int, min_new: int, prompt_len: int, eos_ids) -> torch.Tensor:
+    """The int32[LP_PARAMS] parameter block of the logits processors (host tensor; copy it to the device)."""
+    import struct
+    eos_ids = list(eos_ids)
+    if len(eos_ids) > LP_MAX_EOS:
+        raise NotImplementedError(f"min_new_tokens with more than {LP_MAX_EOS} EOS ids")
+    p = [struct.unpack("<i", struct.pack("<f", float(penalty)))[0], int(ngram), int(min_new), int(prompt_len), len(eos_ids)]
+    p += [int(e) for e in eos_ids] + [0] * (LP_MAX_EOS - len(eos_ids))
+    return torch.tensor(p, dtype=torch.int32)
 
 
 def advance_pos(pos_dev, kv_len_dev, delta: int):
