@@ -12,7 +12,8 @@
  *  - all pointers are DEVICE pointers on the current device unless the name ends in `_host`;
  *    bf16 tensors are `void*`; row-major, innermost dimension contiguous, 16-byte aligned.
  *  - `stream` is a `cudaStream_t` passed as `void*`; every call is asynchronous on that stream.
- *  - no entry point allocates or frees device memory; workspaces are passed in.
+ *  - no entry point allocates or frees device memory; workspaces are passed in.  One exception:
+ *    tl_gemv_bf16 / tl_gemv_bf16_pf allocate their pool of ticket counters (a few KB) once per device.
  *  - return value: 0 on success, a negative `tl_status` otherwise; `tl_last_error()` gives the
  *    (thread-local) message.  There is no CPU fallback: on a machine without an sm_90 device
  *    compute calls return TL_ERR_NO_DEVICE.
@@ -81,7 +82,10 @@ int tl_gemm_bf16_ws_norm(const void* A, const void* B, void* C, int M, int N, in
                          const void* norm_w, float eps, void* H_out, void* stream);
 
 /* ---- decode-shaped Linear (M <= 8 tokens), HBM-bound weight streaming:
- * y[M,N] = f(norm(x)[M,K] * W[N,K]^T).  norm_w != NULL fuses the preceding RMSNorm (K1) as a prologue. */
+ * y[M,N] = f(norm(x)[M,K] * W[N,K]^T).  norm_w != NULL fuses the preceding RMSNorm (K1) as a prologue.
+ * The kernel hands out its rows by ticket from a block of device counter words (see tl_gemv_bf16_ctr); these two
+ * entry points take one from a per-device pool the library allocates at its first call on a device (which therefore
+ * must not be inside a graph capture). */
 int tl_gemv_bf16(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
                  const void* residual, const void* norm_w, float eps, int flags, void* stream);
 /* same, plus a hint: once its own weight loads are issued the kernel queues L2 prefetches of the first next_bytes of
@@ -90,6 +94,14 @@ int tl_gemv_bf16(const void* x, const void* W, void* y, int M, int N, int K, con
 int tl_gemv_bf16_pf(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
                     const void* residual, const void* norm_w, float eps, int flags, const void* next_W,
                     size_t next_bytes, void* stream);
+/* same, with the caller's counter block: TL_GEMV_COUNTER_WORDS device words (4-byte aligned), zero before the first
+ * call; every call leaves them zero.  A call site that owns a block (a launch inside a captured graph) never shares it
+ * with a launch that can run at the same time: the next launch on the stream may start before this one has ended
+ * (programmatic dependent launch).  NULL = a block from the pool. */
+#define TL_GEMV_COUNTER_WORDS 4
+int tl_gemv_bf16_ctr(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
+                     const void* residual, const void* norm_w, float eps, int flags, unsigned* counter,
+                     const void* next_W, size_t next_bytes, void* stream);
 
 /* ---- K3  rotary tables (modeling_qwen2.py:102-113): cos/sin[pos, d/2] = bf16(cos/sin(pos * inv_freq)) */
 int tl_rope_table(const float* inv_freq, void* cos_tab, void* sin_tab, int max_pos, int half_dim, void* stream);
@@ -158,10 +170,11 @@ int tl_attn_bwd_rows(const void* q, const void* k_cache, const void* v_cache, co
 
 /* ---- K7  final norm + lm_head + greedy argmax for M <= 8 rows: ids[m] = argmax_v bf16(norm(x)[m,:]·W[v,:])
  * (lowest index wins ties, as torch.argmax).  logits_out (bf16 [M,V]) optional.
- * workspace >= tl_lmhead_ws(M, V) bytes. */
+ * workspace >= tl_lmhead_ws(M, V) bytes; gemv_counter: the lm_head GEMV's counter block (tl_gemv_bf16_ctr), may be NULL. */
 size_t tl_lmhead_ws(int M, int V);
 int tl_lmhead_argmax(const void* x, const void* W, const void* norm_w, float eps, int64_t* ids_out,
-                     void* logits_out, void* workspace, size_t ws_bytes, int M, int V, int H, void* stream);
+                     void* logits_out, void* workspace, size_t ws_bytes, int M, int V, int H, unsigned* gemv_counter,
+                     void* stream);
 
 /* argmax over bf16 logits[M,V] (any M); workspace >= M*64*8 bytes */
 int tl_argmax_bf16(const void* logits, int64_t* ids_out, void* workspace, size_t ws_bytes, int M, int V, void* stream);

@@ -138,4 +138,19 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
         ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
+// ---------------------------------------------------------------- work tickets
+// A launch hands out its work units in address order from a device counter: a CTA takes n consecutive units at a time,
+// so an SM that streams faster simply takes more and all CTAs finish within one ticket of each other.  The counter
+// words are zero when a launch starts and the last CTA out leaves them zero, so a launch must never share them with
+// another launch that can run at the same time.
+__device__ __forceinline__ int ticket_take(unsigned* ctr, int n) { return (int)atomicAdd(ctr, (unsigned)n); }
+// Called once per CTA, after the CTA's last use of the launch's counters.  True in exactly one CTA, the last to get
+// here, which has already zeroed `exit_word` and must zero the other counters (then __threadfence()).
+__device__ __forceinline__ bool last_cta_out(unsigned* exit_word) {
+    __threadfence();                       // this thread's counter atomics are performed before its exit is counted
+    if (atomicAdd(exit_word, 1u) != gridDim.x - 1) return false;
+    *exit_word = 0u;
+    return true;
+}
+
 }  // namespace tl

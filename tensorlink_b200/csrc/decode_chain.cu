@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(DC_THREADS, 1) decode_chain_kernel(const __gri
             int first_ticket = 0;
             int jn = 0;
             while (jn < p.n_jobs && p.jobs[jn].type != TL_JOB_GEMV) ++jn;
-            if (p.dynamic && jn < p.n_jobs) first_ticket = (int)atomicAdd(&tickets[jn], (unsigned)NW);
+            if (p.dynamic && jn < p.n_jobs) first_ticket = ticket_take(&tickets[jn], NW);
             for (int j = jn; j < p.n_jobs && alive; j = jn) {
                 const tl_decode_job& jb = p.jobs[j];
                 jn = j + 1;
@@ -196,11 +196,11 @@ __global__ void __launch_bounds__(DC_THREADS, 1) decode_chain_kernel(const __gri
                 int base = p.dynamic ? first_ticket : g.u_begin;
                 const int u_end = p.dynamic ? g.U : g.u_end;
                 long long pwait = 0;
-                if (p.dynamic && jn < p.n_jobs) first_ticket = (int)atomicAdd(&tickets[jn], (unsigned)NW);
+                if (p.dynamic && jn < p.n_jobs) first_ticket = ticket_take(&tickets[jn], NW);
                 for (;;) {
                     const bool term = base >= u_end;                 // terminator group: NW empty stages, consumers leave the job
                     int next = base + NW;
-                    if (p.dynamic && !term) next = (int)atomicAdd(&tickets[j], (unsigned)NW);   // used one group later
+                    if (p.dynamic && !term) next = ticket_take(&tickets[j], NW);   // used one group later
                     const int n_c = term ? 1 : g.n_chunks;
                     for (int c = 0; c < n_c && alive; ++c)
                         for (int w = 0; w < NW; ++w) {
@@ -801,15 +801,11 @@ __global__ void __launch_bounds__(DC_THREADS, 1) decode_chain_kernel(const __gri
     // ---- self-cleaning: the last CTA to leave resets the counters for the next launch on this sync slot
     dc_bar(1, DC_CT);
     stamp(DC_MAX_JOBS, 2);
-    if (tid == 0) {            // (a producer parked on an empty-slot wait polls s_dead and leaves by itself)
+    // (a producer parked on an empty-slot wait polls s_dead and leaves by itself)
+    if (tid == 0 && last_cta_out(&p.sync[1])) {
+        p.sync[0] = 0;
+        for (int j = 0; j < p.n_jobs; ++j) p.sync[DC_JOBCTR + j] = 0;
         __threadfence();
-        const unsigned prev = atomicAdd(&p.sync[1], 1u);
-        if (prev == gridDim.x - 1) {
-            p.sync[0] = 0;
-            p.sync[1] = 0;
-            for (int j = 0; j < p.n_jobs; ++j) p.sync[DC_JOBCTR + j] = 0;
-            __threadfence();
-        }
     }
 }
 

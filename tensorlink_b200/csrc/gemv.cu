@@ -6,6 +6,9 @@
 // Algorithmic bytes per launch = 2*N*K (weights) + O(M*(K+N)) activations.
 #include <stdlib.h>
 
+#include <atomic>
+#include <mutex>
+
 #include "common.cuh"
 
 namespace tl {
@@ -217,8 +220,8 @@ static int dispatch_g(int g, int wpi, const void* x, const void* W, void* y, int
 }
 
 int gemv_stream_dispatch(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
-                         const void* residual, const void* norm_w, float eps, int flags, const void* pf_ptr, size_t pf_bytes,
-                         cudaStream_t st);
+                         const void* residual, const void* norm_w, float eps, int flags, unsigned* ctr, const void* pf_ptr,
+                         size_t pf_bytes, cudaStream_t st);
 int gemv_mma_dispatch(const void* x, const void* W, void* y, int M, int N, int K, const void* bias, const void* residual,
                       const void* norm_w, float eps, int flags, cudaStream_t st);
 
@@ -233,20 +236,59 @@ static bool use_stream_kernel() {
 
 }  // namespace tl
 
-extern "C" int tl_gemv_bf16_pf(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
-                               const void* residual, const void* norm_w, float eps, int flags, const void* next_W,
-                               size_t next_bytes, void* stream);
+namespace tl {
 
-extern "C" int tl_gemv_bf16(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
-                            const void* residual, const void* norm_w, float eps, int flags, void* stream) {
-    return tl_gemv_bf16_pf(x, W, y, M, N, K, bias, residual, norm_w, eps, flags, nullptr, 0, stream);
+// Counter blocks for calls that bring none, taken round robin per device.  A block may be handed out again once no
+// launch that used it can still run.  Launches on a stream overlap only through programmatic dependent launch: a launch
+// starts once every CTA of the launch before it is running, and no CTA of it finishes before that launch has completed
+// (the kernels launched this way wait for their predecessor: griddepcontrol.wait).  So the GEMV launches in flight at
+// one time are all resident at once, each with at least one CTA of 288 threads: at most 7 per SM (2048 threads).  One
+// call runs at most 2 launches, on different words of its block.  8 blocks per SM therefore never hand out a block that
+// an earlier call may still be using.  The first call on a device allocates the pool, so it must not be captured.
+constexpr int GEMV_MAX_DEVICES = 64;
+static unsigned* g_ctr_pool[GEMV_MAX_DEVICES];
+static int g_ctr_blocks[GEMV_MAX_DEVICES];
+static std::atomic<unsigned> g_ctr_next[GEMV_MAX_DEVICES];
+static std::mutex g_ctr_mu;
+
+static unsigned* pool_counter() {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= GEMV_MAX_DEVICES) return nullptr;
+    if (!g_ctr_pool[dev]) {
+        std::lock_guard<std::mutex> lk(g_ctr_mu);
+        if (!g_ctr_pool[dev]) {
+            const int n = 8 * sm_count();
+            unsigned* p = nullptr;
+            const size_t bytes = (size_t)n * TL_GEMV_COUNTER_WORDS * sizeof(unsigned);
+            if (cudaMalloc(&p, bytes) != cudaSuccess) return nullptr;
+            if (cudaMemset(p, 0, bytes) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) return nullptr;
+            g_ctr_blocks[dev] = n;
+            g_ctr_pool[dev] = p;
+        }
+    }
+    const unsigned i = g_ctr_next[dev].fetch_add(1u) % (unsigned)g_ctr_blocks[dev];
+    return g_ctr_pool[dev] + (size_t)i * TL_GEMV_COUNTER_WORDS;
 }
+
+}  // namespace tl
 
 extern "C" int tl_gemv_bf16_pf(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
                                const void* residual, const void* norm_w, float eps, int flags, const void* next_W,
                                size_t next_bytes, void* stream) {
+    return tl_gemv_bf16_ctr(x, W, y, M, N, K, bias, residual, norm_w, eps, flags, nullptr, next_W, next_bytes, stream);
+}
+
+extern "C" int tl_gemv_bf16(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
+                            const void* residual, const void* norm_w, float eps, int flags, void* stream) {
+    return tl_gemv_bf16_ctr(x, W, y, M, N, K, bias, residual, norm_w, eps, flags, nullptr, nullptr, 0, stream);
+}
+
+extern "C" int tl_gemv_bf16_ctr(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
+                                const void* residual, const void* norm_w, float eps, int flags, unsigned* counter,
+                                const void* next_W, size_t next_bytes, void* stream) {
     using namespace tl;
     TL_REQUIRE(M >= 1 && M <= 8, TL_ERR_INVALID, "tl_gemv_bf16: M=%d outside 1..8 (use tl_gemm_bf16)", M);
+    TL_REQUIRE(((uintptr_t)counter & 3) == 0, TL_ERR_INVALID, "tl_gemv_bf16: counter block not 4-byte aligned");
     TL_REQUIRE(K % 8 == 0 && N % 2 == 0 && N > 0 && K > 0, TL_ERR_INVALID,
                "tl_gemv_bf16: need K %% 8 == 0 and N even (N=%d K=%d)", N, K);
     TL_REQUIRE(!(flags & ~(TL_EPI_BIAS | TL_EPI_RESIDUAL | TL_EPI_SWIGLU)), TL_ERR_INVALID,
@@ -256,6 +298,12 @@ extern "C" int tl_gemv_bf16_pf(const void* x, const void* W, void* y, int M, int
     TL_REQUIRE(!(flags & TL_EPI_BIAS) || bias, TL_ERR_INVALID, "tl_gemv_bf16: BIAS flag without bias pointer");
     TL_REQUIRE(!(flags & TL_EPI_RESIDUAL) || residual, TL_ERR_INVALID, "tl_gemv_bf16: RESIDUAL flag without pointer");
     cudaStream_t st = (cudaStream_t)stream;
+    if (!counter && use_stream_kernel()) {
+        counter = pool_counter();
+        if (!counter) cudaGetLastError();
+        TL_REQUIRE(counter, TL_ERR_CUDA, "tl_gemv_bf16: allocating the counter pool failed (first call on this device "
+                   "inside a graph capture?)");
+    }
     if (M >= 2 && use_stream_kernel()) {
         // 2..8 rows on mma.sync (gemv_mma.cu): opt-in; its per-row 1-2 KB bulk copies limit how fast an SM can issue
         // them, and it has not been compared with the CUDA-core stream kernel on H100.
@@ -279,9 +327,10 @@ extern "C" int tl_gemv_bf16_pf(const void* x, const void* W, void* y, int M, int
     // the M template is rounded up to 1/2/4/8 and the surplus rows are never written because the epilogue
     // indexes only m < M... (rows beyond M would read x out of bounds), so dispatch exactly for 1..4 and
     // split larger M into two calls.
-    auto run = [&](int m, const bf16* xx, bf16* yy, const bf16* rr, bool last) -> int {
+    // the launches of one call may overlap under programmatic dependent launch: each takes its own two counter words
+    auto run = [&](int m, const bf16* xx, bf16* yy, const bf16* rr, unsigned* ctr, bool last) -> int {
         if (use_stream_kernel()) {
-            const int rc = gemv_stream_dispatch(xx, W, yy, m, N, K, bias, rr, norm_w, eps, flags, last ? next_W : nullptr,
+            const int rc = gemv_stream_dispatch(xx, W, yy, m, N, K, bias, rr, norm_w, eps, flags, ctr, last ? next_W : nullptr,
                                                 last && next_W ? next_bytes : 0, st);
             if (rc != 1) return rc;
         }
@@ -297,7 +346,7 @@ extern "C" int tl_gemv_bf16_pf(const void* x, const void* W, void* y, int M, int
     while (done < M) {
         const int m = (M - done) > 4 ? 4 : (M - done);
         int rc = run(m, (const bf16*)x + (size_t)done * K, (bf16*)y + (size_t)done * n_out,
-                     residual ? (const bf16*)residual + (size_t)done * N : nullptr, done + m == M);
+                     residual ? (const bf16*)residual + (size_t)done * N : nullptr, counter + 2 * (done / 4), done + m == M);
         if (rc != TL_OK) return rc;
         done += m;
     }

@@ -1,13 +1,15 @@
 // Decode-shaped Linear, v2: persistent weight-streaming GEMV with a bulk-copy (TMA) producer warp.
 //
-// One CTA per SM.  Each CTA owns a contiguous range of row PAIRS of W (pair = gate/up for the SwiGLU epilogue)
-// sized so every SM streams the same number of bytes (+-1 pair).  Warp 8 is the producer: it walks the CTA's
-// rows and issues cp.async.bulk copies of <= 16 KB "stages" into a deep shared-memory ring (mbarrier full/empty,
-// ~190 KB in flight per SM), never waiting on the math.  A stage is either P whole consecutive pairs (K small:
-// rows are contiguous in memory, ONE copy) or one K-chunk of one pair (K large: two row-segment copies).  Stages
-// are issued round-robin over the 8 consumer warps; warp w owns every 8th unit for all of its K chunks, so a dot
-// product finishes with one warp reduction and no cross-warp traffic.  x (optionally RMS-normalised with HF
-// rounding) is staged once per CTA while the producer is already streaming.
+// One CTA per SM.  Work is handed out in units: P whole consecutive row PAIRS of W (pair = gate/up for the SwiGLU
+// epilogue) when a pair fits one <= 16 KB ring stage, else one pair in K-chunks of one stage each.  Units are taken in
+// address order from a ticket counter (common.cuh), so an SM that streams faster takes more of them, every CTA finishes
+// within one ticket of the others, and the first units of a launch are the first bytes of W, which the previous launch
+// asked L2 to prefetch.  Warp 8 is the producer: it takes tickets and issues cp.async.bulk copies of the units' stages
+// into a deep shared-memory ring (mbarrier full/empty, ~190 KB in flight per SM), never waiting on the math, and
+// records the unit of every stage beside the barriers.  Ring slot s is always drained by consumer warp s % NW, and a
+// warp takes a whole unit (all of its K chunks, in order), so a dot product finishes with one warp reduction and no
+// cross-warp traffic.  x (optionally RMS-normalised with HF rounding) is staged once per CTA while the producer is
+// already streaming.
 // Algorithmic bytes per launch = 2*N*K.
 #include <stdlib.h>
 
@@ -20,6 +22,11 @@ constexpr int GS_THREADS = (GS_CONSUMER_WARPS + 1) * 32;
 constexpr int GS_MAX_STAGES = 16;
 constexpr int GS_STAGE_BYTES = 16 * 1024;
 constexpr int GS_KC = 4096;            // K chunk (elements) when a pair does not fit one stage
+// Bytes per ticket: one atomic round trip (~1 us under a full HBM stream) has to hide behind the ticket before it, and
+// a CTA finishes at most one ticket after the others.
+constexpr int GS_TICKET_BYTES = 24 * 1024;
+constexpr int GS_SKIP = -2;            // s_unit: an empty stage the warp only hands back
+constexpr int GS_LEAVE = -1;           // s_unit: no units left, the warp leaves
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -29,25 +36,23 @@ template <int M>
 __global__ void __launch_bounds__(GS_THREADS, 1)
 gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16* __restrict__ y, int N, int K,
                    const bf16* __restrict__ bias, const bf16* __restrict__ residual, const bf16* __restrict__ norm_w,
-                   float eps, int flags, int P, int n_stages, int NW, int stage_bytes, const unsigned char* __restrict__ pf_ptr,
-                   unsigned long long pf_bytes) {
+                   float eps, int flags, int P, int n_stages, int NW, int stage_bytes, int G, unsigned* __restrict__ ctr,
+                   const unsigned char* __restrict__ pf_ptr, unsigned long long pf_bytes) {
     extern __shared__ __align__(128) unsigned char smem[];
     unsigned char* ring = smem;                                                    // [n_stages][stage_bytes]
     bf16* xs = reinterpret_cast<bf16*>(smem + (size_t)n_stages * stage_bytes);     // [M][K]
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)n_stages * stage_bytes + (((size_t)M * K * 2 + 15) & ~(size_t)15));
     uint64_t* empty_bar = full_bar + GS_MAX_STAGES;
     __shared__ float s_part[GS_CONSUMER_WARPS][M];
+    __shared__ int s_unit[GS_MAX_STAGES];      // unit in each ring slot (or GS_SKIP / GS_LEAVE), released by the full barrier
 
     // programmatic dependent launch: let the next kernel's CTAs start (and prefetch ITS weights) as SMs free up
     asm volatile("griddepcontrol.launch_dependents;");
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int npairs = N >> 1;
-    const int p_begin = (int)((long long)blockIdx.x * npairs / gridDim.x);
-    const int p_end = (int)((long long)(blockIdx.x + 1) * npairs / gridDim.x);
-    const int n_units = (p_end - p_begin + P - 1) / P;                 // unit = P consecutive pairs
+    const int n_units = (npairs + P - 1) / P;                          // unit = P consecutive pairs
     // NW consumer warps take units; n_stages %% NW == 0, so ring slot s is ALWAYS consumed by warp s %% NW and every
     // waiter observes every phase of the barriers it waits on (no mbarrier parity aliasing).
-    const int n_groups = (n_units + NW - 1) / NW;
     const bool chunked = K > GS_KC || (size_t)K * 4 > GS_STAGE_BYTES;  // a pair does not fit one stage
     const int KC = chunked ? GS_KC : K;
     const int n_chunks = (K + KC - 1) / KC;
@@ -64,34 +69,76 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
     if (warp == GS_CONSUMER_WARPS) {
         // ================================================================= producer (one elected lane)
         if (lane == 0) {
-            int stage = 0;
+            // CTA b's first ticket is units [b*G, (b+1)*G) without a round trip; later tickets come from the counter,
+            // offset by the grid's first tickets.  The next ticket is requested while the current one is handed out.
+            const int first = gridDim.x * G;
+            const bool tickets = first < n_units;          // else the first tickets cover the matrix: no counter traffic
+            int t_cur = blockIdx.x * G, t_used = 0;
+            int t_next = tickets ? first + ticket_take(ctr, G) : n_units;
+            auto next_unit = [&]() -> int {
+                if (t_used == G) {
+                    if (t_next >= n_units) return n_units;
+                    t_cur = t_next;
+                    t_used = 0;
+                    t_next = first + ticket_take(ctr, G);
+                }
+                return t_cur + t_used++;
+            };
+            // per consumer warp: its unit and the next chunk of it.  A chunked unit takes n_chunks of the warp's
+            // stages, so warp w first hands back w*n_chunks/NW empty stages: the warps then need new units at evenly
+            // spread times instead of all at once, and a CTA never commits to NW units in one step.
+            int unit[GS_CONSUMER_WARPS], chunk[GS_CONSUMER_WARPS], skip[GS_CONSUMER_WARPS];
+#pragma unroll
+            for (int w = 0; w < GS_CONSUMER_WARPS; ++w) {
+                unit[w] = 0;
+                chunk[w] = 0;
+                skip[w] = chunked ? w * n_chunks / NW : 0;
+            }
+            int stage = 0, live = NW;
             uint32_t phase = 0;
-            for (int g = 0; g < n_groups; ++g) {
-                for (int c = 0; c < n_chunks; ++c) {
-                    for (int w = 0; w < NW; ++w) {
-                        const int unit = g * NW + w;
+            while (live > 0) {
+#pragma unroll
+                for (int w = 0; w < GS_CONSUMER_WARPS; ++w) {
+                    if (w >= NW) continue;
+                    if (unit[w] != GS_LEAVE) {          // the slots of a warp that left stay untouched
                         mbar_wait(&empty_bar[stage], phase ^ 1);
                         unsigned char* dst = ring + (size_t)stage * stage_bytes;
-                        if (unit >= n_units) {
+                        if (skip[w] > 0) {
+                            --skip[w];
+                            s_unit[stage] = GS_SKIP;
                             mbar_expect_tx(&full_bar[stage], 0);
                         } else {
-                            const int pair0 = p_begin + unit * P;
-                            const int np = min(P, p_end - pair0);
-                            if (!chunked) {      // np pairs = 2*np whole rows, contiguous in memory: one copy
+                            if (chunk[w] == 0) {
+                                unit[w] = next_unit();
+                                if (unit[w] >= n_units) unit[w] = GS_LEAVE;
+                            }
+                            s_unit[stage] = unit[w];
+                            if (unit[w] == GS_LEAVE) {
+                                --live;
+                                mbar_expect_tx(&full_bar[stage], 0);
+                            } else if (!chunked) {   // np pairs = 2*np whole rows, contiguous in memory: one copy
+                                const int pair0 = unit[w] * P;
+                                const int np = min(P, npairs - pair0);
                                 const uint32_t bytes = (uint32_t)(2 * np) * (uint32_t)K * 2u;
                                 mbar_expect_tx(&full_bar[stage], bytes);
                                 bulk_load_1d(dst, W + (size_t)(2 * pair0) * K, bytes, &full_bar[stage]);
-                            } else {             // one K chunk of the two rows of one pair: two copies
-                                const int k0 = c * KC;
+                            } else {                 // one K chunk of the two rows of one pair: two copies
+                                const int k0 = chunk[w] * KC;
                                 const uint32_t bytes = (uint32_t)min(KC, K - k0) * 2u;
                                 mbar_expect_tx(&full_bar[stage], 2 * bytes);
-                                bulk_load_1d(dst, W + (size_t)(2 * pair0) * K + k0, bytes, &full_bar[stage]);
-                                bulk_load_1d(dst + (size_t)KC * 2, W + (size_t)(2 * pair0 + 1) * K + k0, bytes, &full_bar[stage]);
+                                bulk_load_1d(dst, W + (size_t)(2 * unit[w]) * K + k0, bytes, &full_bar[stage]);
+                                bulk_load_1d(dst + (size_t)KC * 2, W + (size_t)(2 * unit[w] + 1) * K + k0, bytes, &full_bar[stage]);
+                                if (++chunk[w] == n_chunks) chunk[w] = 0;
                             }
                         }
-                        if (++stage == n_stages) { stage = 0; phase ^= 1; }
                     }
+                    if (++stage == n_stages) { stage = 0; phase ^= 1; }
                 }
+            }
+            // this CTA takes no more tickets: the last CTA out zeroes the counter for the next launch on these words
+            if (tickets && last_cta_out(ctr + 1)) {
+                ctr[0] = 0u;
+                __threadfence();
             }
             // every load of this CTA is issued (the last ring-full is still in flight): queue L2 prefetches of this
             // CTA's slice of the NEXT kernel's weights behind them, so HBM keeps streaming through this kernel's tail,
@@ -212,46 +259,47 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
                 }
             }
         };
-        // this warp's stages are sequence numbers warp, warp+8, warp+16, ... of the producer's order
-        int seq = warp;
-        for (int g = 0; g < (warp < NW ? n_groups : 0); ++g) {
-            const int unit = g * NW + warp;
-            const bool valid = unit < n_units;
-            const int pair0 = p_begin + unit * P;
-            float a0[M], a1[M];
+        // this warp's stages are sequence numbers warp, warp+NW, warp+2*NW, ... of the producer's order; the producer
+        // says in s_unit which unit each one holds
+        int seq = warp, c = 0;
+        float a0[M], a1[M];
 #pragma unroll
-            for (int m = 0; m < M; ++m) a0[m] = a1[m] = 0.f;
-            for (int c = 0; c < n_chunks; ++c, seq += NW) {
-                const int stage = seq % n_stages;
-                const uint32_t phase = (uint32_t)(seq / n_stages) & 1u;
-                mbar_wait(&full_bar[stage], phase);
-                const unsigned char* src = ring + (size_t)stage * stage_bytes;
-                if (valid) {
-                    if (!chunked) {
-                        const int np = min(P, p_end - pair0);
-                        for (int pp = 0; pp < np; ++pp) {
-                            float b0[M], b1[M];
+        for (int m = 0; m < M; ++m) a0[m] = a1[m] = 0.f;
+        while (warp < NW) {
+            const int stage = seq % n_stages;
+            const uint32_t phase = (uint32_t)(seq / n_stages) & 1u;
+            mbar_wait(&full_bar[stage], phase);
+            const int unit = s_unit[stage];
+            if (unit == GS_LEAVE) break;
+            const unsigned char* src = ring + (size_t)stage * stage_bytes;
+            if (unit >= 0 && !chunked) {
+                const int pair0 = unit * P;
+                const int np = min(P, npairs - pair0);
+                for (int pp = 0; pp < np; ++pp) {
+                    float b0[M], b1[M];
 #pragma unroll
-                            for (int m = 0; m < M; ++m) b0[m] = b1[m] = 0.f;
-                            dot2(reinterpret_cast<const uint4*>(src + (size_t)(2 * pp) * K * 2),
-                                 reinterpret_cast<const uint4*>(src + (size_t)(2 * pp + 1) * K * 2), 0, nvec, b0, b1);
+                    for (int m = 0; m < M; ++m) b0[m] = b1[m] = 0.f;
+                    dot2(reinterpret_cast<const uint4*>(src + (size_t)(2 * pp) * K * 2),
+                         reinterpret_cast<const uint4*>(src + (size_t)(2 * pp + 1) * K * 2), 0, nvec, b0, b1);
 #pragma unroll
-                            for (int m = 0; m < M; ++m) { b0[m] = warp_sum(b0[m]); b1[m] = warp_sum(b1[m]); }
-                            finish(pair0 + pp, b0, b1);
-                        }
-                    } else {
-                        const int k0 = c * KC;
-                        dot2(reinterpret_cast<const uint4*>(src), reinterpret_cast<const uint4*>(src + (size_t)KC * 2), k0,
-                             min(KC, K - k0) >> 3, a0, a1);
-                    }
+                    for (int m = 0; m < M; ++m) { b0[m] = warp_sum(b0[m]); b1[m] = warp_sum(b1[m]); }
+                    finish(pair0 + pp, b0, b1);
                 }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            } else if (unit >= 0) {
+                const int k0 = c * KC;
+                dot2(reinterpret_cast<const uint4*>(src), reinterpret_cast<const uint4*>(src + (size_t)KC * 2), k0,
+                     min(KC, K - k0) >> 3, a0, a1);
             }
-            if (valid && chunked) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            seq += NW;
+            if (unit >= 0 && chunked && ++c == n_chunks) {     // the unit's last chunk: the pair is done
 #pragma unroll
                 for (int m = 0; m < M; ++m) { a0[m] = warp_sum(a0[m]); a1[m] = warp_sum(a1[m]); }
-                finish(pair0, a0, a1);
+                finish(unit, a0, a1);
+#pragma unroll
+                for (int m = 0; m < M; ++m) a0[m] = a1[m] = 0.f;
+                c = 0;
             }
         }
     }
@@ -259,7 +307,8 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
 
 template <int M>
 static int launch_stream(const void* x, const void* W, void* y, int N, int K, const void* bias, const void* residual,
-                         const void* norm_w, float eps, int flags, const void* pf_ptr, size_t pf_bytes, cudaStream_t st) {
+                         const void* norm_w, float eps, int flags, unsigned* ctr, const void* pf_ptr, size_t pf_bytes,
+                         cudaStream_t st) {
     auto kern = gemv_stream_kernel<M>;
     // Two half-size rings per SM (16 consumer warps, finer work split, the next kernel's CTAs become resident as soon as
     // one of the two exits) when an SM's share of W is small — the latency-bound regime of small models; one deep
@@ -292,7 +341,7 @@ static int launch_stream(const void* x, const void* W, void* y, int N, int K, co
     int P = chunked ? 1 : (int)(GS_STAGE_BYTES / ((size_t)K * 4));
     if (P < 1) P = 1;
     if (P > 8) P = 8;
-    // a stage holds exactly one unit: P whole pairs, or one 4096-column chunk of one pair
+    // a stage holds one unit: up to P whole pairs, or one 4096-column chunk of one pair
     const int stage_bytes = chunked ? GS_STAGE_BYTES : (int)((((size_t)P * K * 4) + 127) & ~(size_t)127);
     int max_stages = (int)((SMEM_CAP - fixed) / stage_bytes);
     if (max_stages > GS_MAX_STAGES) max_stages = GS_MAX_STAGES;
@@ -307,6 +356,16 @@ static int launch_stream(const void* x, const void* W, void* y, int N, int K, co
     const int npairs = N >> 1;
     int grid = sm_count() * per_sm;
     if (grid > npairs) grid = npairs;
+    // Few pairs per CTA (the latency-bound launches of small models): one pair per unit and every CTA's first ticket
+    // covers its share, so no CTA waits for a ticket round trip; the split is then as even as a static one.
+    int G;
+    if (npairs <= 8 * grid) {
+        P = 1;
+        G = (npairs + grid - 1) / grid;
+    } else {
+        const int unit_bytes = chunked ? K * 4 : P * K * 4;
+        G = (GS_TICKET_BYTES + unit_bytes - 1) / unit_bytes;
+    }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(GS_THREADS);
@@ -323,22 +382,22 @@ static int launch_stream(const void* x, const void* W, void* y, int N, int K, co
     cfg.attrs = attr;
     cfg.numAttrs = use_pdl ? 1 : 0;
     cudaLaunchKernelEx(&cfg, kern, (const bf16*)x, (const bf16*)W, (bf16*)y, N, K, (const bf16*)bias, (const bf16*)residual,
-                       (const bf16*)norm_w, eps, flags, P, n_stages, NW, stage_bytes, (const unsigned char*)pf_ptr,
+                       (const bf16*)norm_w, eps, flags, P, n_stages, NW, stage_bytes, G, ctr, (const unsigned char*)pf_ptr,
                        (unsigned long long)(pf_bytes & ~(size_t)15));
     return check_launch("tl_gemv_bf16/stream");
 }
 
 // returns TL_OK, an error, or 1 = "not applicable, use the fallback kernel"
 int gemv_stream_dispatch(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
-                         const void* residual, const void* norm_w, float eps, int flags, const void* pf_ptr, size_t pf_bytes,
-                         cudaStream_t st) {
+                         const void* residual, const void* norm_w, float eps, int flags, unsigned* ctr, const void* pf_ptr,
+                         size_t pf_bytes, cudaStream_t st) {
     if (K % 8 != 0 || ((uintptr_t)W & 15)) return 1;
     if ((uintptr_t)pf_ptr & 15) pf_bytes = 0;
     switch (M) {
-        case 1: return launch_stream<1>(x, W, y, N, K, bias, residual, norm_w, eps, flags, pf_ptr, pf_bytes, st);
-        case 2: return launch_stream<2>(x, W, y, N, K, bias, residual, norm_w, eps, flags, pf_ptr, pf_bytes, st);
-        case 3: return launch_stream<3>(x, W, y, N, K, bias, residual, norm_w, eps, flags, pf_ptr, pf_bytes, st);
-        case 4: return launch_stream<4>(x, W, y, N, K, bias, residual, norm_w, eps, flags, pf_ptr, pf_bytes, st);
+        case 1: return launch_stream<1>(x, W, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
+        case 2: return launch_stream<2>(x, W, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
+        case 3: return launch_stream<3>(x, W, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
+        case 4: return launch_stream<4>(x, W, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
         default: return 1;
     }
 }

@@ -111,7 +111,7 @@ int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* 
 }
 
 int tl_lmhead_argmax(const void* x, const void* W, const void* norm_w, float eps, int64_t* ids_out, void* logits_out,
-                     void* workspace, size_t ws_bytes, int M, int V, int H, void* stream) {
+                     void* workspace, size_t ws_bytes, int M, int V, int H, unsigned* gemv_counter, void* stream) {
     using namespace tl;
     TL_REQUIRE(M >= 1 && M <= 8, TL_ERR_INVALID, "tl_lmhead_argmax: M=%d outside 1..8", M);
     TL_REQUIRE(ws_bytes >= tl_lmhead_ws(M, V), TL_ERR_WORKSPACE, "tl_lmhead_argmax: workspace %zu < %zu", ws_bytes,
@@ -119,7 +119,7 @@ int tl_lmhead_argmax(const void* x, const void* W, const void* norm_w, float eps
     unsigned char* ws = (unsigned char*)workspace;
     void* logits = logits_out ? logits_out : (void*)ws;
     size_t off = ((size_t)M * V * sizeof(bf16) + 255) & ~(size_t)255;
-    int rc = tl_gemv_bf16(x, W, logits, M, V, H, nullptr, nullptr, norm_w, eps, 0, stream);
+    int rc = tl_gemv_bf16_ctr(x, W, logits, M, V, H, nullptr, nullptr, norm_w, eps, 0, gemv_counter, nullptr, 0, stream);
     if (rc != TL_OK) return rc;
     return tl_argmax_bf16(logits, ids_out, ws + off, ws_bytes - off, M, V, stream);
 }

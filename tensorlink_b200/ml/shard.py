@@ -223,6 +223,9 @@ class CudaLayerGroup:
         self.n_max = max_tokens or max_batch * max_seq
         self._alloc_bufs(min(self.n_max, 8))
         self.dbufs = self._make_bufs(max_batch)       # decode-time buffers: fixed addresses (captured graphs, job lists)
+        # ticket counters of the four decode GEMVs of every layer (_layer_decode): one block per call site, so no two
+        # launches that can overlap share one, and captured graphs keep fixed addresses
+        self.gemv_ctr = nat.gemv_counters(self.num_layers, 4, device=dev)
         # split-K workspace for batched decode (rows above the GEMV threshold, <= 128): the qkv / o / down Linears have
         # too few output tiles to occupy every SM
         self.gemm_ws = (torch.empty(nat.gemm_splitk_ws(min(max_batch, 128), max(cfg.qkv_dim, cfg.hidden)), dtype=torch.uint8,
@@ -308,13 +311,14 @@ class CudaLayerGroup:
             after = v[f"l{self.layer_ids[j + 1]}.wqkv"]
         else:
             after = self.weights_after_last_layer            # lm_head on the last stage, else layer 0 for the next slot
+        ctr = self.gemv_ctr[j]
         nat.gemv(x, v[f"l{li}.wqkv"], out=w.qkv, bias=v.get(f"l{li}.bqkv"), norm_w=v[f"l{li}.ln1"], eps=cfg.rms_eps,
-                 next_w=v[f"l{li}.wo"])
+                 next_w=v[f"l{li}.wo"], counter=ctr[0])
         self._decode_attention(j, li, B, w)
-        nat.gemv(w.attn, v[f"l{li}.wo"], out=x, residual=x, next_w=v[f"l{li}.wgu"])
+        nat.gemv(w.attn, v[f"l{li}.wo"], out=x, residual=x, next_w=v[f"l{li}.wgu"], counter=ctr[1])
         nat.gemv(x, v[f"l{li}.wgu"], out=w.act, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, flags=nat.EPI_SWIGLU,
-                 next_w=v[f"l{li}.wd"])
-        nat.gemv(w.act, v[f"l{li}.wd"], out=x if out is None else out, residual=x, next_w=after)
+                 next_w=v[f"l{li}.wd"], counter=ctr[2])
+        nat.gemv(w.act, v[f"l{li}.wd"], out=x if out is None else out, residual=x, next_w=after, counter=ctr[3])
 
     def _layer_decode_batched(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor] = None):
         """More single-token rows than the GEMV path takes: wgmma GEMMs in the weight-streaming regime (split along K

@@ -47,6 +47,7 @@ class CudaStage:
                                        dtype=torch.uint8, device=dev)
             self.logits_dec = torch.empty(max_batch, cfg.vocab, dtype=torch.bfloat16, device=dev)
             self.hn = torch.empty(max_batch, cfg.hidden, dtype=torch.bfloat16, device=dev)
+            self.head_ctr = nat.gemv_counters(device=dev)        # the decode lm_head GEMV's ticket counter
             self.sampling: Optional[dict] = None        # set by generate(do_sample=True): temperature / top_k / top_p / seed
             self.sample_ctr = torch.zeros(n_slots, max_batch, dtype=torch.int32, device=dev)
             self.sample_ws: Optional[torch.Tensor] = None
@@ -133,7 +134,8 @@ class CudaStage:
         B = hidden.shape[0]
         logits = self.logits_dec[:B]
         if B <= gemv_max_rows():
-            nat.gemv(hidden, v["head"], out=logits, norm_w=v["norm"], eps=cfg.rms_eps)     # the logits tl_lmhead_argmax makes
+            nat.gemv(hidden, v["head"], out=logits, norm_w=v["norm"], eps=cfg.rms_eps,     # the logits tl_lmhead_argmax makes
+                     counter=self.head_ctr)
         else:
             nat.rmsnorm_fwd(hidden, v["norm"], cfg.rms_eps, out=self.hn[:B])
             nat.gemm(self.hn[:B], v["head"], out=logits)
@@ -149,7 +151,8 @@ class CudaStage:
         cfg, v = self.cfg, self.params.v
         B = hidden.shape[0]
         if B <= gemv_max_rows():
-            nat.lmhead_argmax(hidden, v["head"], v["norm"], cfg.rms_eps, ids_out, self.logits_dec[:B], self.head_ws)
+            nat.lmhead_argmax(hidden, v["head"], v["norm"], cfg.rms_eps, ids_out, self.logits_dec[:B], self.head_ws,
+                              self.head_ctr)
         else:
             nat.rmsnorm_fwd(hidden, v["norm"], cfg.rms_eps, out=self.hn[:B])
             nat.gemm(self.hn[:B], v["head"], out=self.logits_dec[:B])

@@ -39,6 +39,8 @@ _SIGS = {
                              c_float, c_int, c_void_p]),
     "tl_gemv_bf16_pf": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                 c_float, c_int, c_void_p, c_size_t, c_void_p]),
+    "tl_gemv_bf16_ctr": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                 c_float, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "tl_rope_table": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "tl_rope_kv_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -68,7 +70,7 @@ _SIGS = {
     "tl_peer_put": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p]),
     "tl_lmhead_ws": (c_size_t, [c_int, c_int]),
     "tl_lmhead_argmax": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_size_t,
-                                 c_int, c_int, c_int, c_void_p]),
+                                 c_int, c_int, c_int, c_void_p, c_void_p]),
     "tl_argmax_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
     "tl_sample_ws": (c_size_t, [c_int]),
     "tl_sample": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p, c_void_p, c_size_t,
@@ -117,6 +119,7 @@ class DecodeJob(ctypes.Structure):
 JOB_GEMV, JOB_ATTN = 0, 1
 ATTN_POS_PER_ROW = 1
 CHAIN_MAX_JOBS, CHAIN_SYNC_BYTES = 16, 1024
+GEMV_COUNTER_WORDS = 4
 
 _lib: Optional[ctypes.CDLL] = None
 
@@ -259,15 +262,27 @@ _PREFETCH_BYTES = None
 
 
 def prefetch_bytes() -> int:
-    """How much of the next launch's weights a GEMV asks L2 to fetch (TL_PREFETCH_MB, default 8; 0 disables).  The default has not been re-chosen by measurement on H100."""
+    """How much of the next launch's weights a GEMV asks L2 to fetch (TL_PREFETCH_MB, default 8; 0 disables).  The next
+    launch takes its rows in address order, so these are the bytes it reads first.  8 MB measured best on an H100 SXM
+    (700 W) for Qwen2.5-7B decode: 4.89 ms per token against 4.93 at 16 MB and 5.00 at 26 MB, which covers the whole
+    o projection; a larger prefetch competes with the current launch's own stream."""
     global _PREFETCH_BYTES
     if _PREFETCH_BYTES is None:
         _PREFETCH_BYTES = int(float(os.environ.get("TL_PREFETCH_MB", "8")) * (1 << 20))
     return _PREFETCH_BYTES
 
 
+def gemv_counters(*shape, device=None) -> torch.Tensor:
+    """Zeroed counter blocks for GEMV call sites that own one (``[*shape, GEMV_COUNTER_WORDS]`` int32): a captured graph
+    keeps their addresses, and the kernels leave them zero."""
+    return torch.zeros(*shape, GEMV_COUNTER_WORDS, dtype=torch.int32, device=device)
+
+
 def gemv(x: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None, *, bias=None, residual=None,
-         norm_w=None, eps: float = 1e-6, flags: int = 0, next_w: Optional[torch.Tensor] = None) -> torch.Tensor:
+         norm_w=None, eps: float = 1e-6, flags: int = 0, next_w: Optional[torch.Tensor] = None,
+         counter: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``counter``: this call site's block from ``gemv_counters`` (decode call sites inside captured graphs); None
+    takes one from the library's per-device pool."""
     require_device()
     _bf16(x, w, bias, residual, norm_w, out)
     M, K = x.shape
@@ -278,13 +293,9 @@ def gemv(x: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None, *
         flags |= EPI_BIAS
     if residual is not None:
         flags |= EPI_RESIDUAL
-    if next_w is not None and prefetch_bytes() > 0:
-        nb = min(next_w.numel() * next_w.element_size(), prefetch_bytes())
-        _check(load().tl_gemv_bf16_pf(_p(x), _p(w), _p(out), M, N, K, _p(bias), _p(residual), _p(norm_w), eps, flags,
-                                      _p(next_w), nb, _stream()), "tl_gemv_bf16_pf")
-        return out
-    _check(load().tl_gemv_bf16(_p(x), _p(w), _p(out), M, N, K, _p(bias), _p(residual), _p(norm_w), eps, flags,
-                               _stream()), "tl_gemv_bf16")
+    nb = min(next_w.numel() * next_w.element_size(), prefetch_bytes()) if next_w is not None else 0
+    _check(load().tl_gemv_bf16_ctr(_p(x), _p(w), _p(out), M, N, K, _p(bias), _p(residual), _p(norm_w), eps, flags,
+                                   _p(counter), _p(next_w) if nb else None, nb, _stream()), "tl_gemv_bf16_ctr")
     return out
 
 
@@ -358,14 +369,17 @@ def lmhead_ws(M, V) -> int:
     return int(load().tl_lmhead_ws(M, V))
 
 
-def lmhead_argmax(x, w, norm_w, eps, ids_out, logits_out, ws):
+def lmhead_argmax(x, w, norm_w, eps, ids_out, logits_out, ws, counter: Optional[torch.Tensor] = None):
+    """``counter``: the lm_head GEMV's block from ``gemv_counters``, or None for one from the library's pool."""
     require_device()
     _bf16(x, w, norm_w, logits_out)
     M, H = x.shape
     V = w.shape[0]
     assert ids_out.dtype == torch.int64
     _check(load().tl_lmhead_argmax(_p(x), _p(w), _p(norm_w), eps, _p(ids_out), _p(logits_out), _p(ws),
-                                   ws.numel() * ws.element_size(), M, V, H, _stream()), "tl_lmhead_argmax")
+                                   ws.numel() * ws.element_size(), M, V, H,
+                                   _p(counter), _stream()),
+           "tl_lmhead_argmax")
 
 
 def argmax_bf16(logits, ids_out, ws):
