@@ -127,6 +127,15 @@ int tl_attn_decode_fwd(const void* q, const void* k_cache, const void* v_cache, 
                        const int32_t* kv_len_dev, void* workspace, size_t ws_bytes, int B, int n_h, int n_kv,
                        int d, int T_max, float scale, void* stream);
 
+/* ---- K4  verify attention (prompt-lookup decoding): q[q_len, n_h, d] are q_len <= 16 consecutive query tokens of cache
+ * row 0 whose keys and values tl_rope_kv_fwd (S = q_len) already appended at slots *pos_dev .. *pos_dev + q_len - 1.
+ * Query i attends to keys 0..*pos_dev + i; slots above that are never read into an output (they may hold anything,
+ * NaN included).  out[q_len, n_h*d].  Split over the KV length; workspace >= tl_attn_verify_ws(...) bytes. */
+size_t tl_attn_verify_ws(int q_len, int n_h, int d, int T_max);
+int tl_attn_verify_fwd(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* pos_dev,
+                       void* workspace, size_t ws_bytes, int q_len, int n_h, int n_kv, int d, int T_max, float scale,
+                       void* stream);
+
 /* ---- K3 + K4 fused for decode, T_max <= 2048: RoPE (+q/k-norm) of the new token, KV-cache append at *pos_dev and
  * single-pass attention over keys 0..*pos_dev, one launch per layer.  qkv[B, (n_h+2n_kv)*d] post-bias; out[B, n_h*d] */
 int tl_attn_decode_fused(const void* qkv, void* k_cache, void* v_cache, void* out, const int32_t* pos_dev,
@@ -218,6 +227,28 @@ int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* 
 int tl_sample_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
                    const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
                    unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream);
+
+/* ---- prompt-lookup decoding (csrc/prompt_lookup.cu), one row: a verify step runs in_ids[0..K] (the last history token
+ * and K drafts) as K+1 rows and keeps the drafts the model agrees with.  The history is the logits processors' (log, len,
+ * bits above, row 0).  params_dev int32[TL_PL_PARAMS]: the largest n-gram size, max_length (prompt + max_new_tokens:
+ * the history never grows past it), the number of EOS ids and the ids. */
+#define TL_PL_NGRAM 0
+#define TL_PL_MAX_LEN 1
+#define TL_PL_N_EOS 2
+#define TL_PL_EOS 3
+#define TL_PL_MAX_EOS 8
+#define TL_PL_PARAMS (TL_PL_EOS + TL_PL_MAX_EOS)
+#define TL_PL_MAX_DRAFT 15
+/* HF PromptLookupCandidateGenerator.get_candidates on the history: in_ids[0] = its last token, in_ids[1..n] = the
+ * candidates, in_ids[n+1..K] = filler (the last token), *n_cand = n (0..K) */
+int tl_prompt_lookup_draft(const int32_t* log, const int32_t* len, int L, const int32_t* params_dev, int K, int64_t* in_ids,
+                           int32_t* n_cand, void* stream);
+/* ids[0..K]: the model's next token after each of in_ids[0..K].  a = the largest value <= *n_cand with ids[i] ==
+ * in_ids[i+1] for every i < a; e = min(a+1, max_length - len) tokens ids[0..e) join the history and out_log[*count..],
+ * and *count, *pos_dev and *kv_len_dev (= the new *pos_dev) advance by e.  bits may be NULL. */
+int tl_prompt_lookup_accept(const int64_t* ids, const int64_t* in_ids, const int32_t* n_cand, int32_t* log, int32_t* len,
+                            uint32_t* bits, int L, int V, const int32_t* params_dev, int64_t* out_log, int32_t* count,
+                            int out_cap, int32_t* pos_dev, int32_t* kv_len_dev, int K, void* stream);
 
 /* ---- small device-side helpers used by the captured decode graph */
 int tl_advance_pos(int32_t* pos_dev, int32_t* kv_len_dev, int delta, void* stream); /* pos += delta; kv_len = pos */

@@ -2,6 +2,8 @@
 //  * prefill / training forward: flash-style, 64-query x 64-key tiles, warp-level mma.sync for query runs shorter than
 //    one tile; attention_wgmma.cu serves the rest.
 //  * decode: one query per batch row, split over the KV length, HBM-bound on the cache read.
+//  * verify: up to 16 consecutive queries of one row at a device-resident position (prompt-lookup decoding), split the
+//    same way.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -571,6 +573,193 @@ __global__ void attn_decode_reduce_kernel(const float* __restrict__ ws, bf16* __
     out[((size_t)b * n_h + h) * D + dd] = f2bf(L > 0.f ? O / L : 0.f);
 }
 
+// ---- verify: q_len <= 16 query tokens of ONE cache row at slots pos..pos+q_len-1 (their keys and values are already
+// appended), query i attending to keys 0..pos+i.  The idea of attn_decode_mma_kernel carries over: the (query token,
+// head of the GQA group) pairs m = i * n_rep + r are the M rows of mma.sync, n_rep * q_len <= 128 of them, 64 per CTA
+// (grid.z = 2 when there are more: the second CTA re-reads the split's K/V through L2).  Each of the 4 warps owns 16 rows
+// and every key of a 64-key tile; a CTA covers DEC_CHUNK_MMA keys through the same 2-tile cp.async ring.  Keys at or
+// above pos + q_len are never loaded (zero-filled), keys above pos + i are masked out of row i, so whatever the cache
+// holds there (stale drafts, NaN) never reaches an output.  Partial record per (kv head, split, row m): m, l, o[D].
+constexpr int VER_MAX_Q = 16;
+
+template <int D>
+__global__ void __launch_bounds__(FA_THREADS) attn_verify_mma_kernel(const bf16* __restrict__ q, const bf16* __restrict__ k_cache,
+                                                                      const bf16* __restrict__ v_cache, float* __restrict__ ws,
+                                                                      const int32_t* __restrict__ pos_dev, int q_len, int n_h,
+                                                                      int n_kv, int T_max, int n_splits, float scale_log2) {
+    constexpr int LDS = D + 8;
+    constexpr int CPR = D / 8;
+    const int split = blockIdx.x, kvh = blockIdx.y, m0 = blockIdx.z * FA_BQ;
+    const int pos = *pos_dev;
+    const int kv_total = min(pos + q_len, T_max);
+    const int c0 = split * DEC_CHUNK_MMA;
+    if (c0 >= kv_total) return;
+    const int n_rep = n_h / n_kv, M = n_rep * q_len;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    bf16* sQ = reinterpret_cast<bf16*>(smem_raw);          // [64][LDS]
+    bf16* sK = sQ + FA_BQ * LDS;                           // [2][64][LDS]
+    bf16* sV = sK + 2 * FA_BKV * LDS;                      // [2][64][LDS]
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int g = lane >> 2, t4 = lane & 3;
+    const bf16* kg = k_cache + (size_t)kvh * T_max * D;
+    const bf16* vg = v_cache + (size_t)kvh * T_max * D;
+    for (int c = tid; c < FA_BQ * CPR; c += FA_THREADS) {
+        const int r = c / CPR, cc = c - r * CPR, m = m0 + r;
+        const bool ok = m < M;
+        const int i = ok ? m / n_rep : 0, h = kvh * n_rep + (ok ? m - i * n_rep : 0);
+        cp_async16(sQ + r * LDS + cc * 8, q + ((size_t)i * n_h + h) * D + cc * 8, ok);
+    }
+    const int n_tiles = min(DEC_CHUNK_MMA / FA_BKV, (kv_total - c0 + FA_BKV - 1) / FA_BKV);
+    auto load_tile = [&](int t) {
+        const int kv0 = c0 + t * FA_BKV, buf = t & 1;
+        for (int c = tid; c < FA_BKV * CPR; c += FA_THREADS) {
+            const int r = c / CPR, cc = c - r * CPR;
+            const bool ok = (kv0 + r) < kv_total;
+            const size_t off = (size_t)(ok ? kv0 + r : 0) * D + cc * 8;
+            cp_async16(sK + (buf * FA_BKV + r) * LDS + cc * 8, kg + off, ok);
+            cp_async16(sV + (buf * FA_BKV + r) * LDS + cc * 8, vg + off, ok);
+        }
+        cp_async_commit();                                  // (the q rows ride in the first group)
+    };
+    load_tile(0);
+    if (1 < n_tiles) load_tile(1);
+    const bool active = m0 + warp * 16 < M;                 // a warp whose 16 rows are all padding only loads
+    int last[2];                                            // last key of rows g and g+8 (-1: padding row)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int m = m0 + warp * 16 + g + r * 8;
+        last[r] = m < M ? min(pos + m / n_rep, kv_total - 1) : -1;
+    }
+    float o[D / 8][4];
+#pragma unroll
+    for (int i = 0; i < D / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    uint32_t qf[D / 16][4];
+    for (int t = 0; t < n_tiles; ++t) {
+        if (t + 1 < n_tiles) cp_async_wait<1>(); else cp_async_wait<0>();
+        __syncthreads();
+        if (active) {
+            if (t == 0) {
+#pragma unroll
+                for (int ks = 0; ks < D / 16; ++ks)
+                    ldmatrix_x4(qf[ks], sQ + (warp * 16 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8);
+            }
+            const bf16* sKb = sK + (t & 1) * FA_BKV * LDS;
+            const bf16* sVb = sV + (t & 1) * FA_BKV * LDS;
+            float s[FA_BKV / 8][4];
+#pragma unroll
+            for (int i = 0; i < FA_BKV / 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
+#pragma unroll
+            for (int ks = 0; ks < D / 16; ++ks) {
+#pragma unroll
+                for (int np = 0; np < FA_BKV / 16; ++np) {
+                    uint32_t bfr[4];
+                    const int mi = lane >> 3;
+                    ldmatrix_x4(bfr, sKb + (np * 16 + (mi >> 1) * 8 + (lane & 7)) * LDS + ks * 16 + (mi & 1) * 8);
+                    mma_bf16_16816(s[2 * np], qf[ks], bfr[0], bfr[1]);
+                    mma_bf16_16816(s[2 * np + 1], qf[ks], bfr[2], bfr[3]);
+                }
+            }
+            const int kv0 = c0 + t * FA_BKV;
+            float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+            for (int i = 0; i < FA_BKV / 8; ++i) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int key = kv0 + i * 8 + 2 * t4 + (e & 1);
+                    const float v = key <= last[e >> 1] ? s[i][e] * scale_log2 : -INFINITY;
+                    s[i][e] = v;
+                    mx[e >> 1] = fmaxf(mx[e >> 1], v);
+                }
+            }
+            float alpha[2], msub[2];
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+                mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+                const float m_new = fmaxf(m_run[r], mx[r]);
+                msub[r] = (m_new == -INFINITY) ? 0.f : m_new;
+                alpha[r] = exp2f(m_run[r] - msub[r]);
+                m_run[r] = m_new;
+            }
+            float rs[2] = {0.f, 0.f};
+            uint32_t pf[FA_BKV / 16][4];
+#pragma unroll
+            for (int i = 0; i < FA_BKV / 8; ++i) {
+                const float p0 = exp2f(s[i][0] - msub[0]), p1 = exp2f(s[i][1] - msub[0]);
+                const float p2 = exp2f(s[i][2] - msub[1]), p3 = exp2f(s[i][3] - msub[1]);
+                rs[0] += p0 + p1;
+                rs[1] += p2 + p3;
+                pf[i >> 1][(i & 1) * 2] = pack_bf16(p0, p1);          // P is cast to bf16 before P.V (SDPA contract)
+                pf[i >> 1][(i & 1) * 2 + 1] = pack_bf16(p2, p3);
+            }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                rs[r] += __shfl_xor_sync(0xffffffffu, rs[r], 1);
+                rs[r] += __shfl_xor_sync(0xffffffffu, rs[r], 2);
+                l_run[r] = l_run[r] * alpha[r] + rs[r];
+            }
+#pragma unroll
+            for (int i = 0; i < D / 8; ++i) {
+                o[i][0] *= alpha[0];
+                o[i][1] *= alpha[0];
+                o[i][2] *= alpha[1];
+                o[i][3] *= alpha[1];
+            }
+#pragma unroll
+            for (int kk = 0; kk < FA_BKV / 16; ++kk) {
+#pragma unroll
+                for (int dp = 0; dp < D / 16; ++dp) {
+                    uint32_t bfr[4];
+                    const int mi = lane >> 3;
+                    ldmatrix_x4_trans(bfr, sVb + (kk * 16 + (mi & 1) * 8 + (lane & 7)) * LDS + dp * 16 + (mi >> 1) * 8);
+                    mma_bf16_16816(o[2 * dp], pf[kk], bfr[0], bfr[1]);
+                    mma_bf16_16816(o[2 * dp + 1], pf[kk], bfr[2], bfr[3]);
+                }
+            }
+        }
+        if (t + 2 < n_tiles) {
+            __syncthreads();                                // every warp is done with this buffer
+            load_tile(t + 2);
+        }
+    }
+    if (!active) return;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int m = m0 + warp * 16 + g + r * 8;
+        if (m >= M) continue;
+        float* rec = ws + (((size_t)kvh * n_splits + split) * M + m) * (2 + D);
+        if (t4 == 0) { rec[0] = m_run[r]; rec[1] = l_run[r]; }
+#pragma unroll
+        for (int i = 0; i < D / 8; ++i)
+            *reinterpret_cast<float2*>(rec + 2 + i * 8 + 2 * t4) = make_float2(o[i][2 * r], o[i][2 * r + 1]);
+    }
+}
+
+// one CTA per (query head, query token): merges the splits that hold keys 0..pos+i (the later splits were computed for
+// the later tokens only and are not read)
+template <int D>
+__global__ void attn_verify_reduce_kernel(const float* __restrict__ ws, bf16* __restrict__ out, const int32_t* __restrict__ pos_dev,
+                                          int q_len, int n_h, int n_kv, int T_max, int n_splits) {
+    const int h = blockIdx.x, i = blockIdx.y, dd = threadIdx.x;
+    const int n_rep = n_h / n_kv, kvh = h / n_rep, M = n_rep * q_len, m = i * n_rep + (h - kvh * n_rep);
+    const int last = min(*pos_dev + i, T_max - 1);
+    const int ns = min(n_splits, last / DEC_CHUNK_MMA + 1);
+    const float* base = ws + ((size_t)kvh * n_splits * M + m) * (2 + D);
+    const size_t step = (size_t)M * (2 + D);
+    float Mx = -INFINITY;
+    for (int s = 0; s < ns; ++s) Mx = fmaxf(Mx, base[s * step]);
+    float L = 0.f, O = 0.f;
+    for (int s = 0; s < ns; ++s) {
+        const float* rec = base + s * step;
+        if (rec[0] == -INFINITY) continue;
+        const float w = exp2f(rec[0] - Mx);
+        L += rec[1] * w;
+        O += rec[2 + dd] * w;
+    }
+    out[((size_t)i * n_h + h) * D + dd] = f2bf(L > 0.f ? O / L : 0.f);
+}
+
 }  // namespace tl
 
 namespace tl {
@@ -652,6 +841,44 @@ int tl_attn_decode_fwd_rows(const void* q, const void* k_cache, const void* v_ca
     TL_REQUIRE(kv_start_dev != nullptr, TL_ERR_INVALID, "tl_attn_decode_fwd_rows: kv_start_dev is null");
     return attn_decode_launch(q, k_cache, v_cache, out, kv_len_dev, workspace, ws_bytes, B, n_h, n_kv, d, T_max, scale,
                               kv_start_dev, (cudaStream_t)stream, "tl_attn_decode_fwd_rows");
+}
+
+size_t tl_attn_verify_ws(int q_len, int n_h, int d, int T_max) {
+    const size_t n_splits = (size_t)(T_max + tl::DEC_CHUNK_MMA - 1) / tl::DEC_CHUNK_MMA;
+    return n_splits * (size_t)n_h * (size_t)(q_len > 0 ? q_len : 0) * (2 + d) * sizeof(float);
+}
+
+int tl_attn_verify_fwd(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* pos_dev,
+                       void* workspace, size_t ws_bytes, int q_len, int n_h, int n_kv, int d, int T_max, float scale,
+                       void* stream) {
+    using namespace tl;
+    const char* what = "tl_attn_verify_fwd";
+    TL_REQUIRE(d == 64 || d == 128, TL_ERR_INVALID, "%s: head_dim %d not in {64,128}", what, d);
+    TL_REQUIRE(n_kv > 0 && n_h % n_kv == 0 && n_h / n_kv <= DEC_MAX_REP, TL_ERR_INVALID,
+               "%s: GQA group %d/%d unsupported (max %d)", what, n_h, n_kv, DEC_MAX_REP);
+    TL_REQUIRE(q_len >= 1 && q_len <= VER_MAX_Q, TL_ERR_INVALID, "%s: q_len %d not in [1, %d]", what, q_len, VER_MAX_Q);
+    TL_REQUIRE(q && k_cache && v_cache && out && pos_dev && workspace, TL_ERR_INVALID, "%s: null argument", what);
+    TL_REQUIRE(T_max >= q_len, TL_ERR_INVALID, "%s: T_max %d < q_len %d", what, T_max, q_len);
+    TL_REQUIRE(ws_bytes >= tl_attn_verify_ws(q_len, n_h, d, T_max), TL_ERR_WORKSPACE,
+               "%s: workspace %zu < %zu", what, ws_bytes, tl_attn_verify_ws(q_len, n_h, d, T_max));
+    const int n_splits = (T_max + DEC_CHUNK_MMA - 1) / DEC_CHUNK_MMA;
+    const int M = n_h / n_kv * q_len;
+    const dim3 g1(n_splits, n_kv, (M + FA_BQ - 1) / FA_BQ), g2(n_h, q_len);
+    const float sl2 = scale * 1.4426950408889634f;
+    const size_t smem = (size_t)(FA_BQ + 4 * FA_BKV) * (d + 8) * sizeof(bf16);
+    cudaStream_t st = (cudaStream_t)stream;
+#define TL_VERIFY(D_)                                                                                                       \
+    do {                                                                                                                    \
+        static bool done = false;                                                                                           \
+        if (!done) { cudaFuncSetAttribute(attn_verify_mma_kernel<D_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); done = true; } \
+        attn_verify_mma_kernel<D_><<<g1, FA_THREADS, smem, st>>>((const bf16*)q, (const bf16*)k_cache, (const bf16*)v_cache,     \
+                                                                 (float*)workspace, pos_dev, q_len, n_h, n_kv, T_max, n_splits, sl2); \
+        attn_verify_reduce_kernel<D_><<<g2, D_, 0, st>>>((const float*)workspace, (bf16*)out, pos_dev, q_len, n_h, n_kv, T_max, \
+                                                         n_splits);                                                         \
+    } while (0)
+    if (d == 64) TL_VERIFY(64); else TL_VERIFY(128);
+#undef TL_VERIFY
+    return check_launch(what);
 }
 
 }  // extern "C"

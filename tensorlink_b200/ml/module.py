@@ -22,7 +22,7 @@ from typing import Any, Callable, Dict, Optional, Union
 
 import torch
 
-from ..native import LP_MAX_EOS
+from ..native import LP_MAX_EOS, PL_MAX_DRAFT, PL_MAX_EOS
 from ..p2p.link import StageLink, init_process_group_from_env
 from . import graphing
 from .configs import ShardModelConfig, get_config
@@ -91,6 +91,42 @@ def _logits_processors(repetition_penalty=None, no_repeat_ngram_size=None, min_n
     if len(eos) > LP_MAX_EOS:
         raise NotImplementedError(f"min_new_tokens with {len(eos)} EOS ids (at most {LP_MAX_EOS})")
     return {"penalty": float(p), "ngram": int(n), "min_new": int(k), "eos": eos}
+
+
+def _prompt_lookup(num_tokens, ngram, shape, max_new, max_seq, sampling=None, procs=None, world=1, stage=None,
+                   eos_token_id=None) -> Optional[dict]:
+    """HF's ``prompt_lookup_num_tokens`` / ``max_matching_ngram_size`` as {K, ngram}, or None when prompt lookup is off
+    (``num_tokens`` None).  ``shape``: the [rows, S] of the prompt that reaches the cache.  Values HF rejects, more than
+    PL_MAX_DRAFT drafts, more than one row, or a cache too short for the last verify step raise ValueError; what the
+    verify step does not implement (sampling, logits processors, several stages, another stage than the CUDA one,
+    more EOS ids than the device parameter block holds) raises NotImplementedError."""
+    if num_tokens is None:
+        return None
+    n = 2 if ngram is None else ngram
+    for name, v in (("prompt_lookup_num_tokens", num_tokens), ("max_matching_ngram_size", n)):
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral) or v < 1:
+            raise ValueError(f"{name} has to be a positive integer, but is {v!r}")
+    K = int(num_tokens)
+    if K > PL_MAX_DRAFT:
+        raise ValueError(f"prompt_lookup_num_tokens={K}: a verify step runs at most {PL_MAX_DRAFT} drafts")
+    rows, S = shape
+    if rows != 1:
+        raise ValueError(f"prompt lookup decoding generates one row at a time, got {rows} rows")
+    if S + max_new + K > max_seq:
+        raise ValueError(f"prompt lookup needs S + max_new_tokens + prompt_lookup_num_tokens <= max_seq (the last verify "
+                         f"step writes K+1 cache slots); got {S} + {max_new} + {K} > {max_seq}")
+    if sampling is not None:
+        raise NotImplementedError("prompt_lookup_num_tokens with do_sample=True (drafts are verified greedily)")
+    if procs is not None:
+        raise NotImplementedError("prompt_lookup_num_tokens with repetition_penalty / no_repeat_ngram_size / min_new_tokens")
+    if world > 1:
+        raise NotImplementedError("prompt_lookup_num_tokens on a pipeline of more than one stage")
+    if len(_eos_list(eos_token_id)) > PL_MAX_EOS:
+        raise NotImplementedError(f"prompt_lookup_num_tokens with more than {PL_MAX_EOS} EOS ids")
+    from .stage import CudaStage
+    if not isinstance(stage, CudaStage):
+        raise NotImplementedError("prompt_lookup_num_tokens needs the CUDA stage")
+    return {"K": K, "ngram": int(n)}
 
 
 def _check_attention_mask(mask, shape):
@@ -473,6 +509,49 @@ class DistributedModel(torch.nn.Module):
             self.link.broadcast(out, 0)              # every rank returns the whole result, prompt and pads included
         return out
 
+    def _generate_lookup(self, input_ids, max_new, streamer, use_graph, lookup):
+        """Greedy generation of one row with prompt-lookup drafts (``_prompt_lookup``) on the one CUDA stage: prefill, the
+        first token from the head, then verify steps (ml/stage.py ``prompt_lookup_step``), each drafting K tokens from
+        the row's history on the device and emitting 1..K+1 tokens.  The host replays rounds of
+        r = max(1, (max_new - count) // (K+1)) steps (at most EOS_CHECK_EVERY with ``eos_token_id``), so no step runs
+        once max_new tokens are out, and reads the token count once per round."""
+        st, dev = self.stage, self.device
+        K = lookup["K"]
+        S = input_ids.shape[1]
+        st.set_sampling(None)                      # greedy, no logits processors: the plain argmax head
+        st.set_logits_processors(None)
+        t0 = time.perf_counter()
+        ids = input_ids.to(dev)
+        x = st.prefill(st.embed(ids), 0, 0)
+        first = st.ids_dec[0][:1]
+        st.head_argmax(x[:, -1, :].contiguous(), first, 0)
+        eos_ids = _eos_list(self._eos[0])
+        steps, count = 0, 0
+        tokens = torch.zeros(0, dtype=torch.int64)
+        if max_new >= 1:
+            st.prompt_lookup_begin(torch.cat([ids, first.view(1, 1)], dim=1), K, lookup["ngram"], S + max_new, eos_ids)
+            while True:
+                count = st.prompt_lookup_count()
+                new = st.prompt_lookup_tokens(tokens.numel(), count)
+                tokens = torch.cat([tokens, new])
+                if streamer is not None:
+                    for j in range(new.numel()):
+                        streamer.put(new[j:j + 1])
+                if count >= max_new or any(int(t) in eos_ids for t in new):
+                    break
+                r = max(1, (max_new - count) // (K + 1))
+                if eos_ids:
+                    r = min(r, EOS_CHECK_EVERY)
+                for _ in range(r):
+                    st.prompt_lookup_step(use_graph)
+                steps += r
+        self.timers["prompt_lookup_steps"] = steps
+        result = torch.cat([ids, tokens[:max_new].to(dev).view(1, -1)], dim=1)
+        if streamer is not None:
+            streamer.end()
+        self.timers["generate_wall_s"] = time.perf_counter() - t0
+        return apply_eos(result, S, *self._eos)
+
     # ------------------------------------------------------------------------------------------ generate
     @torch.no_grad()
     def generate(self, *args, **kwargs) -> Optional[torch.Tensor]:
@@ -490,7 +569,11 @@ class DistributedModel(torch.nn.Module):
         pad in every row are dropped, and each row's pad slots are masked out of attention with its RoPE positions
         starting at its first real token.  The result keeps HF's layout [pads | prompt | new tokens | pad_token_id...].
         With ``do_sample`` a padded batch draws one stream per micro-batch slot, exactly as an unpadded batch does, so
-        a row's tokens depend on the seed and its place in the batch, not on its prompt length."""
+        a row's tokens depend on the seed and its place in the batch, not on its prompt length.
+        ``prompt_lookup_num_tokens=K`` (1..15; ``max_matching_ngram_size`` n, default 2): HF's prompt-lookup decoding for
+        one greedy row on one stage.  Each step drafts up to K tokens that followed an earlier occurrence of the last
+        n-gram and verifies them with the current token as K+1 rows in one pass over the weights (csrc/prompt_lookup.cu);
+        the output is greedy decoding's.  ``self.timers["prompt_lookup_steps"]`` counts the verify steps."""
         input_ids = kwargs.pop("input_ids", args[0] if args else None)
         max_new = int(kwargs.pop("max_new_tokens", 20))
         streamer = kwargs.pop("streamer", None)
@@ -508,6 +591,8 @@ class DistributedModel(torch.nn.Module):
         procs = _logits_processors(kwargs.pop("repetition_penalty", None), kwargs.pop("no_repeat_ngram_size", None),
                                    kwargs.pop("min_new_tokens", None), self._eos[0])
         mask = kwargs.pop("attention_mask", None)
+        lookup = kwargs.pop("prompt_lookup_num_tokens", None)
+        ngram = kwargs.pop("max_matching_ngram_size", None) if lookup is not None else None
         _check_unconsumed(kwargs, "DistributedModel.generate")
         link, st, cfg = self.link, self.stage, self.cfg
         groups, padded = None, None
@@ -523,6 +608,13 @@ class DistributedModel(torch.nn.Module):
             else:
                 g = _left_pad_groups(mask)
                 groups = None if g is None else (g, tuple(input_ids.shape))
+        if lookup is not None:
+            lookup = _prompt_lookup(lookup, ngram, tuple(input_ids.shape) if input_ids is not None else (1, 0), max_new,
+                                    self.max_seq, sampling, procs, self.world, st, self._eos[0])
+            result = self._generate_lookup(input_ids, max_new, streamer, use_graph, lookup)
+            if padded is not None and padded[0].shape[1]:
+                result = torch.cat([padded[0].to(result.device), result], dim=1)
+            return result
         if self.world > 1:
             groups, padded, procs = link.broadcast_object((groups, padded, procs))
         if procs is not None and not hasattr(st, "set_logits_processors"):

@@ -233,6 +233,8 @@ class CudaLayerGroup:
         self.dec_ws = torch.empty(max(nat.attn_decode_ws(max_batch, cfg.n_heads, cfg.head_dim, max_seq), 16),
                                   dtype=torch.uint8, device=dev)
         self.scale = cfg.head_dim ** -0.5
+        self.vbufs: Optional[ShardBuffers] = None     # verify step (verify_step_inplace): its own buffers, on first use
+        self.ver_gemm_ws = self.ver_attn_ws = None
         self.allow_chain = True              # DistributedModel clears it when NCCL kernels share the device during decode
         self.chain_sync: Optional[torch.Tensor] = None
         self.chain_attn_ws: Optional[torch.Tensor] = None
@@ -302,9 +304,12 @@ class CudaLayerGroup:
         nat.attn_decode_fwd(w.q, self.kc[j], self.vc[j], w.attn, self.kvlen_dev, self.dec_ws, B, cfg.n_heads,
                             cfg.n_kv_heads, cfg.head_dim, self.scale, kv_start=ks)
 
-    def _layer_decode(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor] = None):
-        """Same layer for B <= 8 single-token rows: weight-streaming GEMVs with the norms fused as prologues."""
+    def _layer_decode(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor] = None,
+                      attention=None):
+        """Same layer for B <= 8 single-token rows: weight-streaming GEMVs with the norms fused as prologues.
+        ``attention``: what turns w.qkv into w.attn instead of ``_decode_attention`` (the verify step's)."""
         cfg, v, li = self.cfg, self.p.v, self.layer_ids[j]
+        attention = attention or self._decode_attention
         # every GEMV names the weights of the launch after it: it queues L2 prefetches behind its own loads, so HBM keeps
         # streaming through the launch boundary (and through the attention kernel) instead of idling there
         if j + 1 < self.num_layers:
@@ -314,22 +319,25 @@ class CudaLayerGroup:
         ctr = self.gemv_ctr[j]
         nat.gemv(x, v[f"l{li}.wqkv"], out=w.qkv, bias=v.get(f"l{li}.bqkv"), norm_w=v[f"l{li}.ln1"], eps=cfg.rms_eps,
                  next_w=v[f"l{li}.wo"], counter=ctr[0])
-        self._decode_attention(j, li, B, w)
+        attention(j, li, B, w)
         nat.gemv(w.attn, v[f"l{li}.wo"], out=x, residual=x, next_w=v[f"l{li}.wgu"], counter=ctr[1])
         nat.gemv(x, v[f"l{li}.wgu"], out=w.act, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, flags=nat.EPI_SWIGLU,
                  next_w=v[f"l{li}.wd"], counter=ctr[2])
         nat.gemv(w.act, v[f"l{li}.wd"], out=x if out is None else out, residual=x, next_w=after, counter=ctr[3])
 
-    def _layer_decode_batched(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor] = None):
+    def _layer_decode_batched(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor] = None,
+                              attention=None, ws: Optional[torch.Tensor] = None):
         """More single-token rows than the GEMV path takes: wgmma GEMMs in the weight-streaming regime (split along K
         where a Linear has too few output tiles to occupy every SM) + decode attention.  The RMSNorm after each
-        residual Linear rides in that Linear's split-K reduce pass, so layer j > 0 finds its normalised input in w.h."""
+        residual Linear rides in that Linear's split-K reduce pass, so layer j > 0 finds its normalised input in w.h.
+        ``attention`` / ``ws``: the verify step's attention and split-K workspace instead of the decode ones."""
         cfg, v, li = self.cfg, self.p.v, self.layer_ids[j]
-        ws = self.gemm_ws if B <= 128 else None
+        if ws is None:
+            ws = self.gemm_ws if B <= 128 else None
         if j == 0:
             nat.rmsnorm_fwd(x, v[f"l{li}.ln1"], cfg.rms_eps, out=w.h)
         nat.gemm(w.h, v[f"l{li}.wqkv"], out=w.qkv, bias=v.get(f"l{li}.bqkv"), ws=ws)
-        self._decode_attention(j, li, B, w)
+        (attention or self._decode_attention)(j, li, B, w)
         nat.gemm(w.attn, v[f"l{li}.wo"], out=x, residual=x, ws=ws, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, h_out=w.h)
         nat.gemm(w.h, v[f"l{li}.wgu"], out=w.act, flags=nat.EPI_SWIGLU, ws=ws)
         if j + 1 < self.num_layers:
@@ -393,6 +401,42 @@ class CudaLayerGroup:
                 self._layer_decode_batched(j, x, B, w, o)
         if advance:
             nat.advance_pos(self.pos_dev, None, 1)
+
+    # ------------------------------------------------------------------------------------------ verify step
+    def _verify_attention(self, j: int, li: int, n: int, w: ShardBuffers):
+        """w.qkv (post-bias) of n consecutive tokens of cache row 0 -> w.attn: RoPE + append at pos..pos+n-1, then
+        token i attends to keys 0..pos+i."""
+        cfg, v = self.cfg, self.p.v
+        nat.rope_kv_fwd(w.qkv, w.q, self.kc[j], self.vc[j], self.pos_dev, self.cos, self.sin, v.get(f"l{li}.qn"),
+                        v.get(f"l{li}.kn"), cfg.rms_eps, n, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim)
+        nat.attn_verify_fwd(w.q, self.kc[j], self.vc[j], w.attn, self.pos_dev, self.ver_attn_ws, n, cfg.n_heads,
+                            cfg.n_kv_heads, cfg.head_dim, self.scale)
+
+    def verify_step_inplace(self, x: torch.Tensor):
+        """x [n,H] (n <= 16): n consecutive tokens of cache row 0 at positions pos_dev.., updated in place through this
+        shard's layers, as one graph-capturable launch sequence.  ``decode_step_inplace`` for n rows of one sequence:
+        the same Linears (GEMVs up to gemv_max_rows(), else the split-K GEMMs), the per-kernel sequence always, and the
+        verify attention.  Neither pos_dev nor kvlen_dev moves here (the accept step advances both).  The buffers are
+        this step's own, at fixed addresses, allocated on first use; the GEMV ticket counters are the decode step's
+        (each launch leaves its block zeroed, and a verify step never overlaps a decode step)."""
+        n = x.shape[0]
+        if not 1 <= n <= nat.VERIFY_MAX_ROWS:
+            raise ValueError(f"verify step takes 1..{nat.VERIFY_MAX_ROWS} rows, got {n}")
+        if self.ragged:
+            raise NotImplementedError("verify step on a left-padded slot")
+        if self.vbufs is None:
+            cfg, dev, R = self.cfg, self.device, nat.VERIFY_MAX_ROWS
+            self.vbufs = self._make_bufs(R)
+            self.ver_gemm_ws = torch.empty(nat.gemm_splitk_ws(R, max(cfg.qkv_dim, cfg.hidden)), dtype=torch.uint8, device=dev)
+            self.ver_attn_ws = torch.empty(nat.attn_verify_ws(R, cfg.n_heads, cfg.head_dim, self.T_max), dtype=torch.uint8,
+                                           device=dev)
+        b = self.vbufs
+        w = ShardBuffers(b.x[:n], b.h[:n], b.qkv[:n], b.q[:n], b.attn[:n], b.act[:n])
+        for j in range(self.num_layers):
+            if n <= gemv_max_rows():
+                self._layer_decode(j, x, n, w, attention=self._verify_attention)
+            else:
+                self._layer_decode_batched(j, x, n, w, attention=self._verify_attention, ws=self.ver_gemm_ws)
 
     # ------------------------------------------------------------------------------------------ chained decode step
     def chain_ok(self, B: int) -> bool:

@@ -57,6 +57,9 @@ class CudaStage:
             self.lp_flags = 0
             self.hist_log: Optional[torch.Tensor] = None
             self.hist_len = self.hist_bits = self.lp_params = self.lp_ws = None
+            # prompt-lookup decoding (prompt_lookup_begin): the verify step's buffers, allocated on first use
+            self.pl: Optional[dict] = None
+            self.pl_K = 0
 
     # ------------------------------------------------------------------------------------------ pieces
     def embed(self, ids: torch.Tensor) -> torch.Tensor:
@@ -99,17 +102,24 @@ class CudaStage:
         self.procs, self.lp_flags = procs, flags
         if procs is None:
             return
-        n_slots, dev, V = len(self.slots), self.device, self.cfg.vocab
+        dev, V = self.device, self.cfg.vocab
         if self.lp_ws is None:
             self.lp_ws = torch.empty(nat.logits_proc_ws(self.max_batch, V), dtype=torch.uint8, device=dev)
             self.lp_params = torch.zeros(nat.LP_PARAMS, dtype=torch.int32, device=dev)
+        self._ensure_history(length)
+        self.lp_params.copy_(nat.lp_params(procs["penalty"], procs["ngram"], procs["min_new"], procs["prompt_len"],
+                                           procs["eos"] if procs["min_new"] > 0 else []))
+
+    def _ensure_history(self, length: int):
+        """The token history of every slot and row, holding at least ``length`` tokens (the logits processors' and
+        prompt lookup's)."""
+        n_slots, dev, V = len(self.slots), self.device, self.cfg.vocab
+        if self.hist_len is None:
             self.hist_len = torch.zeros(n_slots, self.max_batch, dtype=torch.int32, device=dev)
             self.hist_bits = torch.zeros(n_slots, self.max_batch, (V + 31) // 32, dtype=torch.int32, device=dev)
         if self.hist_log is None or self.hist_log.shape[2] < length:
             self.hist_log = torch.zeros(n_slots, self.max_batch, max(length, self.max_seq), dtype=torch.int32, device=dev)
             self.graphs.clear()                      # the captured kernels hold the old log's address
-        self.lp_params.copy_(nat.lp_params(procs["penalty"], procs["ngram"], procs["min_new"], procs["prompt_len"],
-                                           procs["eos"] if procs["min_new"] > 0 else []))
 
     def fill_history(self, slot: int, prompt: torch.Tensor):
         """Row r of ``slot`` starts its token history with ``prompt[r]`` (int64 [b, S] on this device, pad columns included)."""
@@ -225,6 +235,111 @@ class CudaStage:
             # capture does not execute; state is still the saved one
             self.graphs[key] = g
         g.replay()
+
+    # ------------------------------------------------------------------------------------------ prompt-lookup decoding
+    def prompt_lookup_begin(self, seq: torch.Tensor, K: int, ngram: int, max_length: int, eos=()):
+        """Start a prompt-lookup run of slot 0, row 0 right after its prefill: ``seq`` (int64 [1, S+1] on this device) is
+        the prompt and the first generated token, whose key is not cached yet (pos_dev = S).  The row's history becomes
+        ``seq`` and the output log starts with the first token (count 1).  Each verify step then drafts K tokens from
+        the history (largest n-gram ``ngram``, EOS ids ``eos``) and runs K+1 rows; the history never grows past
+        ``max_length`` (prompt + max_new_tokens)."""
+        if not (self.has_embed and self.has_head) or len(self.slots[0].layer_ids) != self.cfg.n_layers:
+            raise NotImplementedError("prompt lookup decoding runs on a stage that holds the whole model")
+        if not 1 <= K <= nat.PL_MAX_DRAFT:
+            raise ValueError(f"prompt lookup drafts 1..{nat.PL_MAX_DRAFT} tokens per step, got {K}")
+        dev, H, V, R = self.device, self.cfg.hidden, self.cfg.vocab, nat.VERIFY_MAX_ROWS
+        if self.pl is None:
+            self.pl = {"in_ids": torch.zeros(R, dtype=torch.int64, device=dev),       # last token + drafts (+ filler)
+                       "ids": torch.zeros(R, dtype=torch.int64, device=dev),          # the model's token after each row
+                       "n_cand": torch.zeros(1, dtype=torch.int32, device=dev),
+                       "count": torch.zeros(1, dtype=torch.int32, device=dev),        # tokens in the output log
+                       "params": torch.zeros(nat.PL_PARAMS, dtype=torch.int32, device=dev),
+                       "x": torch.zeros(R, H, dtype=torch.bfloat16, device=dev),
+                       "hn": torch.zeros(R, H, dtype=torch.bfloat16, device=dev),
+                       "logits": torch.zeros(R, V, dtype=torch.bfloat16, device=dev),
+                       "head_ws": torch.empty(max(nat.lmhead_ws(8, V), R * 64 * 8 + 256), dtype=torch.uint8, device=dev),
+                       "out_log": torch.zeros(0, dtype=torch.int64, device=dev)}
+        pl = self.pl
+        S = seq.shape[1] - 1
+        if pl["out_log"].numel() < max_length - S:
+            pl["out_log"] = torch.zeros(max(max_length - S, 64), dtype=torch.int64, device=dev)
+            self.graphs.clear()                      # the captured accept kernel holds the old log's address
+        self._ensure_history(max_length)
+        self.fill_history(0, seq.contiguous())
+        pl["params"].copy_(nat.pl_params(ngram, max_length, eos))
+        pl["out_log"][:1].copy_(seq[0, -1:])
+        pl["count"].fill_(1)
+        self.pl_K = int(K)
+
+    def _verify_body(self, draft: bool = True):
+        """draft -> embed K+1 ids -> layers -> final norm + lm_head + argmax of every row -> accept."""
+        pl, grp, cfg, v = self.pl, self.slots[0], self.cfg, self.params.v
+        K = self.pl_K
+        n = K + 1
+        log, length, bits = self.hist_log[0, 0], self.hist_len[0, :1], self.hist_bits[0, 0]
+        if draft:
+            nat.pl_draft(log, length, pl["params"], K, pl["in_ids"], pl["n_cand"])
+        x, ids = pl["x"][:n], pl["ids"][:n]
+        nat.embed_fwd(pl["in_ids"][:n], v["embed"], out=x)
+        grp.verify_step_inplace(x)
+        if n <= gemv_max_rows():
+            nat.lmhead_argmax(x, v["head"], v["norm"], cfg.rms_eps, ids, pl["logits"][:n], pl["head_ws"], self.head_ctr)
+        else:
+            nat.rmsnorm_fwd(x, v["norm"], cfg.rms_eps, out=pl["hn"][:n])
+            nat.gemm(pl["hn"][:n], v["head"], out=pl["logits"][:n])
+            nat.argmax_bf16(pl["logits"][:n], ids, pl["head_ws"])
+        nat.pl_accept(ids, pl["in_ids"], pl["n_cand"], log, length, bits, cfg.vocab, pl["params"], pl["out_log"], pl["count"],
+                      grp.pos_dev, grp.kvlen_dev, K)
+
+    def prompt_lookup_step(self, use_graph: bool = True):
+        """One verify step (``prompt_lookup_begin``), as ONE graph launch per K: it emits 1..K+1 tokens into the output
+        log, or none once the history holds max_length tokens."""
+        if not use_graph:
+            self._verify_body()
+            return
+        key = ("verify", self.pl_K + 1)
+        g = self.graphs.get(key)
+        if g is None:
+            # warm up outside capture (first-use buffers, attributes), restoring what it touches
+            grp, pl = self.slots[0], self.pl
+            state = (grp.pos_dev, grp.kvlen_dev, pl["count"], pl["in_ids"], pl["n_cand"], self.hist_len, self.hist_bits)
+            saved = [t.clone() for t in state]
+            side = torch.cuda.Stream(device=self.device)
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                self._verify_body()
+            torch.cuda.current_stream().wait_stream(side)
+            for t, s in zip(state, saved):
+                t.copy_(s)
+            torch.cuda.synchronize(self.device)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._verify_body()
+            self.graphs[key] = g
+        g.replay()
+
+    def prompt_lookup_count(self) -> int:
+        """Tokens in the output log (synchronises with the device)."""
+        return int(self.pl["count"].item())
+
+    def prompt_lookup_tokens(self, start: int, end: int) -> torch.Tensor:
+        """Output-log entries start..end-1 (int64, on the host)."""
+        return self.pl["out_log"][start:end].cpu()
+
+    def verify_drafts(self, drafts) -> List[int]:
+        """One eager verify step with the caller's drafts (at most K) in place of the history's: in_ids = [last history
+        token, *drafts, filler].  Returns the tokens it emitted: the accepted drafts and the model's next token."""
+        pl = self.pl
+        K = self.pl_K
+        if len(drafts) > K:
+            raise ValueError(f"{len(drafts)} drafts for a verify step of K={K}")
+        nat.pl_draft(self.hist_log[0, 0], self.hist_len[0, :1], pl["params"], K, pl["in_ids"], pl["n_cand"])
+        if drafts:
+            pl["in_ids"][1:1 + len(drafts)].copy_(torch.as_tensor(list(drafts), dtype=torch.int64))
+        pl["n_cand"].fill_(len(drafts))
+        c0 = self.prompt_lookup_count()
+        self._verify_body(draft=False)
+        return self.prompt_lookup_tokens(c0, self.prompt_lookup_count()).tolist()
 
     def check(self):
         for g in self.slots:

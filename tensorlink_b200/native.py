@@ -50,6 +50,11 @@ _SIGS = {
     "tl_attn_decode_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_int,
                                    c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "tl_attn_decode_fused": (c_int, [c_void_p] * 9 + [c_float, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+    "tl_attn_verify_ws": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "tl_attn_verify_fwd": (c_int, [c_void_p] * 6 + [c_size_t, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+    "tl_prompt_lookup_draft": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "tl_prompt_lookup_accept": (c_int, [c_void_p] * 6 + [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                                         c_void_p, c_int, c_void_p]),
     "tl_rope_kv_fwd_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "tl_attn_prefill_fwd_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
@@ -365,6 +370,24 @@ def attn_decode_fwd(q, k_cache, v_cache, out, kv_len_dev, ws, B, n_h, n_kv, d, s
                                           _stream()), "tl_attn_decode_fwd_rows")
 
 
+VERIFY_MAX_ROWS = 16
+
+
+def attn_verify_ws(q_len, n_h, d, T_max) -> int:
+    return int(load().tl_attn_verify_ws(q_len, n_h, d, T_max))
+
+
+def attn_verify_fwd(q, k_cache, v_cache, out, pos_dev, ws, q_len, n_h, n_kv, d, scale):
+    """q [q_len, n_h*d] at cache slots pos..pos+q_len-1 of row 0 (already appended) -> out [q_len, n_h*d]; query i sees
+    keys 0..pos+i."""
+    require_device()
+    _bf16(q, k_cache, v_cache, out)
+    assert pos_dev.dtype == torch.int32
+    _check(load().tl_attn_verify_fwd(_p(q), _p(k_cache), _p(v_cache), _p(out), _p(pos_dev), _p(ws),
+                                     ws.numel() * ws.element_size(), q_len, n_h, n_kv, d, k_cache.shape[2], scale, _stream()),
+           "tl_attn_verify_fwd")
+
+
 def lmhead_ws(M, V) -> int:
     return int(load().tl_lmhead_ws(M, V))
 
@@ -467,6 +490,48 @@ def lp_params(penalty: float, ngram: int, min_new: int, prompt_len: int, eos_ids
     p = [struct.unpack("<i", struct.pack("<f", float(penalty)))[0], int(ngram), int(min_new), int(prompt_len), len(eos_ids)]
     p += [int(e) for e in eos_ids] + [0] * (LP_MAX_EOS - len(eos_ids))
     return torch.tensor(p, dtype=torch.int32)
+
+
+PL_NGRAM, PL_MAX_LEN, PL_N_EOS, PL_EOS, PL_MAX_EOS = 0, 1, 2, 3, 8
+PL_PARAMS = PL_EOS + PL_MAX_EOS
+PL_MAX_DRAFT = 15
+
+
+def pl_params(ngram: int, max_length: int, eos_ids) -> torch.Tensor:
+    """The int32[PL_PARAMS] parameter block of prompt-lookup decoding (host tensor; copy it to the device)."""
+    eos_ids = list(eos_ids)
+    if len(eos_ids) > PL_MAX_EOS:
+        raise NotImplementedError(f"prompt lookup with more than {PL_MAX_EOS} EOS ids")
+    p = [int(ngram), int(max_length), len(eos_ids)] + [int(e) for e in eos_ids] + [0] * (PL_MAX_EOS - len(eos_ids))
+    return torch.tensor(p, dtype=torch.int32)
+
+
+def _i32(*ts):
+    for t in ts:
+        if t.dtype != torch.int32 or not t.is_cuda or not t.is_contiguous():
+            raise NativeError("contiguous int32 CUDA tensor expected")
+
+
+def pl_draft(log, length, params, K: int, in_ids, n_cand):
+    """Row 0's history (log int32 [L], length int32 [1]) -> in_ids int64 [K+1] (last token, drafts, filler), n_cand."""
+    require_device()
+    _i32(log, length, params, n_cand)
+    assert in_ids.dtype == torch.int64 and in_ids.numel() >= K + 1 and params.numel() >= PL_PARAMS
+    _check(load().tl_prompt_lookup_draft(_p(log), _p(length), log.shape[-1], _p(params), K, _p(in_ids), _p(n_cand),
+                                         _stream()), "tl_prompt_lookup_draft")
+
+
+def pl_accept(ids, in_ids, n_cand, log, length, bits, V: int, params, out_log, count, pos_dev, kv_len_dev, K: int):
+    """The agreeing drafts of a verify step and the model's next token join the history and ``out_log``."""
+    require_device()
+    _i32(n_cand, log, length, params, count, pos_dev, kv_len_dev)
+    assert ids.dtype == torch.int64 and in_ids.dtype == torch.int64 and out_log.dtype == torch.int64
+    assert ids.numel() >= K + 1 and in_ids.numel() >= K + 1 and params.numel() >= PL_PARAMS
+    if bits is not None and bits.shape[-1] != (V + 31) // 32:
+        raise NativeError(f"history bitmap has {bits.shape[-1]} words per row, V={V} needs {(V + 31) // 32}")
+    _check(load().tl_prompt_lookup_accept(_p(ids), _p(in_ids), _p(n_cand), _p(log), _p(length), _p(bits), log.shape[-1], V,
+                                          _p(params), _p(out_log), _p(count), out_log.numel(), _p(pos_dev), _p(kv_len_dev),
+                                          K, _stream()), "tl_prompt_lookup_accept")
 
 
 def advance_pos(pos_dev, kv_len_dev, delta: int):
