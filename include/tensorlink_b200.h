@@ -249,6 +249,11 @@ int tl_prompt_lookup_draft(const int32_t* log, const int32_t* len, int L, const 
 int tl_prompt_lookup_accept(const int64_t* ids, const int64_t* in_ids, const int32_t* n_cand, int32_t* log, int32_t* len,
                             uint32_t* bits, int L, int V, const int32_t* params_dev, int64_t* out_log, int32_t* count,
                             int out_cap, int32_t* pos_dev, int32_t* kv_len_dev, int K, void* stream);
+/* assisted decoding (an assistant model drafts in_ids[1..K]), one row: with P = *len - 1, the history's log[P-1], log[P]
+ * -> asst_in[0..1] (the assistant's 2-row catch-up at cache slots P-1, P), log[P] -> in_ids[0], and the assistant's
+ * *asst_pos = *asst_kv_len = P - 1.  Nothing else is written. */
+int tl_assist_prep(const int32_t* log, const int32_t* len, int L, int64_t* asst_in, int64_t* in_ids, int32_t* asst_pos,
+                   int32_t* asst_kv_len, void* stream);
 
 /* ---- small device-side helpers used by the captured decode graph */
 int tl_advance_pos(int32_t* pos_dev, int32_t* kv_len_dev, int delta, void* stream); /* pos += delta; kv_len = pos */

@@ -11,6 +11,8 @@
 //                     filler], n_cand = the number of candidates
 //   * accept kernel   one warp: a = the agreeing prefix of the candidates; ids[0..a] join the history and the output
 //                     log, the count, the cache position and the KV length advance by a+1.
+//   * assist prep     one thread: with an assistant model as the draft source (assisted decoding), its catch-up input
+//                     and cache position for the round, and the target's current token.
 #include <limits.h>
 
 #include "common.cuh"
@@ -94,9 +96,33 @@ __global__ void pl_accept_kernel(const int64_t* __restrict__ ids, const int64_t*
     }
 }
 
+// Assisted decoding: a second (smaller) model drafts the K tokens.  Every round starts with a 2-row catch-up of the
+// assistant at cache slots P-1 and P (P = len - 1, the slot of the last history token): slot P-1 is the one it never fed
+// when all K drafts of the previous round were accepted, slot P may hold a rejected draft.  Its drafts then overwrite
+// any slot above P that still holds one, so this and the positions are the whole rollback.
+__global__ void assist_prep_kernel(const int32_t* __restrict__ log, const int32_t* __restrict__ len_dev, int L_cap,
+                                   int64_t* __restrict__ asst_in, int64_t* __restrict__ in_ids,
+                                   int32_t* __restrict__ asst_pos, int32_t* __restrict__ asst_kv_len) {
+    const int P = max(min(*len_dev, L_cap) - 1, 1);       // the history holds the prompt and one token at least
+    asst_in[0] = log[P - 1];
+    asst_in[1] = log[P];
+    in_ids[0] = log[P];
+    *asst_pos = P - 1;
+    *asst_kv_len = P - 1;
+}
+
 }  // namespace tl
 
 extern "C" {
+
+int tl_assist_prep(const int32_t* log, const int32_t* len, int L, int64_t* asst_in, int64_t* in_ids, int32_t* asst_pos,
+                   int32_t* asst_kv_len, void* stream) {
+    using namespace tl;
+    TL_REQUIRE(log && len && asst_in && in_ids && asst_pos && asst_kv_len, TL_ERR_INVALID, "tl_assist_prep: null argument");
+    TL_REQUIRE(L >= 2, TL_ERR_INVALID, "tl_assist_prep: bad shape L=%d", L);
+    assist_prep_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(log, len, L, asst_in, in_ids, asst_pos, asst_kv_len);
+    return check_launch("tl_assist_prep");
+}
 
 int tl_prompt_lookup_draft(const int32_t* log, const int32_t* len, int L, const int32_t* params_dev, int K, int64_t* in_ids,
                            int32_t* n_cand, void* stream) {

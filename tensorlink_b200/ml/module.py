@@ -61,7 +61,9 @@ def _config_from_hf(model) -> ShardModelConfig:
 _NEUTRAL_KW = {"use_cache": (True, False, None), "return_dict": (True, None), "output_attentions": (False, None),
                "output_hidden_states": (False, None), "num_beams": (1, None), "num_return_sequences": (1, None),
                "repetition_penalty": (1.0, None), "past_key_values": (None,), "position_ids": (None,),
-               "return_dict_in_generate": (False, None), "logits_to_keep": (0, None), "min_new_tokens": (0, None)}
+               "return_dict_in_generate": (False, None), "logits_to_keep": (0, None), "min_new_tokens": (0, None),
+               # assisted decoding drafts a fixed K per captured verify step: no schedule, no confidence cut
+               "num_assistant_tokens_schedule": ("constant", None), "assistant_confidence_threshold": (None,)}
 
 
 def _check_unconsumed(kwargs: dict, what: str):
@@ -127,6 +129,56 @@ def _prompt_lookup(num_tokens, ngram, shape, max_new, max_seq, sampling=None, pr
     if not isinstance(stage, CudaStage):
         raise NotImplementedError("prompt_lookup_num_tokens needs the CUDA stage")
     return {"K": K, "ngram": int(n)}
+
+
+# num_assistant_tokens when the keyword is absent: the K with the most expected tokens per ms in tools/bench_assisted.py
+# (Qwen2.5-7B target, Qwen2.5-0.5B assistant, one H100), with an ASSUMED agreement of 0.8 per draft token between the two
+# models.  It changes speed only, never the output.
+ASSISTED_DEFAULT_K = 2
+
+
+def _device_key(d):
+    """(type, index) of a device, "cuda" meaning the current CUDA device."""
+    d = torch.device(d)
+    return d.type, (torch.cuda.current_device() if d.type == "cuda" and d.index is None else d.index)
+
+
+def _assisted(target, assistant, num_tokens, shape, max_new, sampling=None, procs=None) -> dict:
+    """HF's ``assistant_model`` / ``num_assistant_tokens`` as {K, ngram, assistant (its stage)}.  A non-DistributedModel
+    raises TypeError; the target as its own assistant, a bad K (1..PL_MAX_DRAFT), more than one row or a cache of either
+    model too short for the last verify step raise ValueError; what the verify step does not implement (sampling,
+    logits processors, several stages on either side, a stage other than the CUDA one, an assistant on another device)
+    raises NotImplementedError."""
+    if not isinstance(assistant, DistributedModel):
+        raise TypeError(f"assistant_model has to be a DistributedModel, got {type(assistant).__name__}; wrap an HF "
+                        "module as DistributedModel(hf_model, training=False)")
+    if assistant is target:
+        raise ValueError("assistant_model is the model itself (the two would share one KV cache)")
+    K = ASSISTED_DEFAULT_K if num_tokens is None else num_tokens
+    if isinstance(K, bool) or not isinstance(K, numbers.Integral) or not 1 <= K <= PL_MAX_DRAFT:
+        raise ValueError(f"num_assistant_tokens has to be an integer in 1..{PL_MAX_DRAFT} (a verify step runs at most "
+                         f"{PL_MAX_DRAFT} drafts), but is {num_tokens!r}")
+    K = int(K)
+    rows, S = shape
+    if rows != 1:
+        raise ValueError(f"assisted decoding generates one row at a time, got {rows} rows")
+    for who, m in (("the model", target), ("the assistant", assistant)):
+        if S + max_new + K > m.max_seq:
+            raise ValueError(f"assisted decoding needs S + max_new_tokens + num_assistant_tokens <= max_seq of {who} (the "
+                             f"last verify step writes K+1 cache slots); got {S} + {max_new} + {K} > {m.max_seq}")
+    if sampling is not None:
+        raise NotImplementedError("assistant_model with do_sample=True (drafts are verified greedily)")
+    if procs is not None:
+        raise NotImplementedError("assistant_model with repetition_penalty / no_repeat_ngram_size / min_new_tokens")
+    if target.world > 1 or assistant.world > 1:
+        raise NotImplementedError("assistant_model with a model or an assistant on a pipeline of more than one stage")
+    from .stage import CudaStage
+    if not isinstance(target.stage, CudaStage) or not isinstance(assistant.stage, CudaStage):
+        raise NotImplementedError("assistant_model needs the CUDA stage on the model and on the assistant")
+    if _device_key(assistant.stage.device) != _device_key(target.stage.device):
+        raise NotImplementedError(f"assistant_model on {assistant.stage.device} for a model on {target.stage.device} "
+                                  "(both run on one device)")
+    return {"K": K, "ngram": 0, "assistant": assistant.stage}
 
 
 def _check_attention_mask(mask, shape):
@@ -510,13 +562,14 @@ class DistributedModel(torch.nn.Module):
         return out
 
     def _generate_lookup(self, input_ids, max_new, streamer, use_graph, lookup):
-        """Greedy generation of one row with prompt-lookup drafts (``_prompt_lookup``) on the one CUDA stage: prefill, the
-        first token from the head, then verify steps (ml/stage.py ``prompt_lookup_step``), each drafting K tokens from
-        the row's history on the device and emitting 1..K+1 tokens.  The host replays rounds of
+        """Greedy generation of one row with prompt-lookup drafts (``_prompt_lookup``) or an assistant's (``_assisted``)
+        on the one CUDA stage: prefill, the first token from the head, then verify steps (ml/stage.py
+        ``prompt_lookup_step``), each drafting K tokens on the device (from the row's history, or by the assistant,
+        whose cache starts with the prompt's prefill) and emitting 1..K+1 tokens.  The host replays rounds of
         r = max(1, (max_new - count) // (K+1)) steps (at most EOS_CHECK_EVERY with ``eos_token_id``), so no step runs
         once max_new tokens are out, and reads the token count once per round."""
         st, dev = self.stage, self.device
-        K = lookup["K"]
+        K, asst = lookup["K"], lookup.get("assistant")
         S = input_ids.shape[1]
         st.set_sampling(None)                      # greedy, no logits processors: the plain argmax head
         st.set_logits_processors(None)
@@ -529,7 +582,10 @@ class DistributedModel(torch.nn.Module):
         steps, count = 0, 0
         tokens = torch.zeros(0, dtype=torch.int64)
         if max_new >= 1:
-            st.prompt_lookup_begin(torch.cat([ids, first.view(1, 1)], dim=1), K, lookup["ngram"], S + max_new, eos_ids)
+            if asst is not None:
+                asst.prefill(asst.embed(ids), 0, 0)
+            st.prompt_lookup_begin(torch.cat([ids, first.view(1, 1)], dim=1), K, lookup["ngram"], S + max_new, eos_ids,
+                                   assistant=asst)
             while True:
                 count = st.prompt_lookup_count()
                 new = st.prompt_lookup_tokens(tokens.numel(), count)
@@ -545,7 +601,7 @@ class DistributedModel(torch.nn.Module):
                 for _ in range(r):
                     st.prompt_lookup_step(use_graph)
                 steps += r
-        self.timers["prompt_lookup_steps"] = steps
+        self.timers["prompt_lookup_steps" if asst is None else "assisted_steps"] = steps
         result = torch.cat([ids, tokens[:max_new].to(dev).view(1, -1)], dim=1)
         if streamer is not None:
             streamer.end()
@@ -573,7 +629,19 @@ class DistributedModel(torch.nn.Module):
         ``prompt_lookup_num_tokens=K`` (1..15; ``max_matching_ngram_size`` n, default 2): HF's prompt-lookup decoding for
         one greedy row on one stage.  Each step drafts up to K tokens that followed an earlier occurrence of the last
         n-gram and verifies them with the current token as K+1 rows in one pass over the weights (csrc/prompt_lookup.cu);
-        the output is greedy decoding's.  ``self.timers["prompt_lookup_steps"]`` counts the verify steps."""
+        the output is greedy decoding's.  ``self.timers["prompt_lookup_steps"]`` counts the verify steps.
+        ``assistant_model=draft`` (another ``DistributedModel`` on this device, one stage; wrap an HF module as
+        ``DistributedModel(hf_model, training=False)``), ``num_assistant_tokens=K`` (1..15): HF's assisted decoding with
+        greedy selection, for one greedy row on one stage.  Each step the assistant greedily drafts K tokens and the model
+        verifies them with its current token as K+1 rows in one pass over its weights, keeping the agreeing prefix and
+        its own next token, all on the GPU; the output is greedy decoding's.  The two models may differ in every
+        dimension, the vocabulary included: an id one of them cannot embed reads its embedding row 0, which can only
+        cost acceptance, since a draft is kept only where it equals the model's own argmax.  Matching tokenizers are the
+        caller's responsibility, as in HF.  Without ``num_assistant_tokens`` K is ASSISTED_DEFAULT_K, the K with the
+        most expected tokens per ms on an H100 for a Qwen2.5-7B model and a Qwen2.5-0.5B assistant ASSUMING an
+        agreement of 0.8 per draft token (not measured on real checkpoints); it changes speed only, never the output.
+        ``num_assistant_tokens_schedule`` may only be "constant" and ``assistant_confidence_threshold`` only None.
+        ``self.timers["assisted_steps"]`` counts the verify steps."""
         input_ids = kwargs.pop("input_ids", args[0] if args else None)
         max_new = int(kwargs.pop("max_new_tokens", 20))
         streamer = kwargs.pop("streamer", None)
@@ -593,7 +661,12 @@ class DistributedModel(torch.nn.Module):
         mask = kwargs.pop("attention_mask", None)
         lookup = kwargs.pop("prompt_lookup_num_tokens", None)
         ngram = kwargs.pop("max_matching_ngram_size", None) if lookup is not None else None
+        assistant = kwargs.pop("assistant_model", None)
+        n_assist = kwargs.pop("num_assistant_tokens", None) if assistant is not None else None
         _check_unconsumed(kwargs, "DistributedModel.generate")
+        if assistant is not None and lookup is not None:
+            # (HF drafts by prompt lookup here and ignores the assistant without a word)
+            raise NotImplementedError("assistant_model together with prompt_lookup_num_tokens: pick one draft source")
         link, st, cfg = self.link, self.stage, self.cfg
         groups, padded = None, None
         if link.first and mask is not None:
@@ -608,9 +681,12 @@ class DistributedModel(torch.nn.Module):
             else:
                 g = _left_pad_groups(mask)
                 groups = None if g is None else (g, tuple(input_ids.shape))
-        if lookup is not None:
+        if assistant is not None:
+            lookup = _assisted(self, assistant, n_assist, tuple(input_ids.shape), max_new, sampling, procs)
+        elif lookup is not None:
             lookup = _prompt_lookup(lookup, ngram, tuple(input_ids.shape) if input_ids is not None else (1, 0), max_new,
                                     self.max_seq, sampling, procs, self.world, st, self._eos[0])
+        if lookup is not None:
             result = self._generate_lookup(input_ids, max_new, streamer, use_graph, lookup)
             if padded is not None and padded[0].shape[1]:
                 result = torch.cat([padded[0].to(result.device), result], dim=1)

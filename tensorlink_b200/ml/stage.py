@@ -7,7 +7,7 @@ in-process by ``DistributedModel`` and neighbours are reached through ``StageLin
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -57,9 +57,13 @@ class CudaStage:
             self.lp_flags = 0
             self.hist_log: Optional[torch.Tensor] = None
             self.hist_len = self.hist_bits = self.lp_params = self.lp_ws = None
-            # prompt-lookup decoding (prompt_lookup_begin): the verify step's buffers, allocated on first use
+            # prompt-lookup decoding (prompt_lookup_begin): the verify step's buffers, allocated on first use; the draft
+            # source is the history's n-grams, or an assistant stage (assisted decoding)
             self.pl: Optional[dict] = None
             self.pl_K = 0
+            self.pl_assistant: Optional["CudaStage"] = None
+            # as an assistant (assist_draft): its 2-row catch-up input and hidden rows, allocated on first use
+            self.asst: Optional[dict] = None
 
     # ------------------------------------------------------------------------------------------ pieces
     def embed(self, ids: torch.Tensor) -> torch.Tensor:
@@ -237,16 +241,33 @@ class CudaStage:
         g.replay()
 
     # ------------------------------------------------------------------------------------------ prompt-lookup decoding
-    def prompt_lookup_begin(self, seq: torch.Tensor, K: int, ngram: int, max_length: int, eos=()):
+    def _whole_model(self) -> bool:
+        return self.has_embed and self.has_head and len(self.slots[0].layer_ids) == self.cfg.n_layers
+
+    def prompt_lookup_begin(self, seq: torch.Tensor, K: int, ngram: int, max_length: int, eos=(),
+                            assistant: Optional["CudaStage"] = None):
         """Start a prompt-lookup run of slot 0, row 0 right after its prefill: ``seq`` (int64 [1, S+1] on this device) is
         the prompt and the first generated token, whose key is not cached yet (pos_dev = S).  The row's history becomes
         ``seq`` and the output log starts with the first token (count 1).  Each verify step then drafts K tokens from
         the history (largest n-gram ``ngram``, EOS ids ``eos``) and runs K+1 rows; the history never grows past
-        ``max_length`` (prompt + max_new_tokens)."""
-        if not (self.has_embed and self.has_head) or len(self.slots[0].layer_ids) != self.cfg.n_layers:
+        ``max_length`` (prompt + max_new_tokens).
+        ``assistant``: assisted decoding instead.  That stage (another model on this device, its slot 0 prefilled with
+        the prompt) drafts K tokens greedily in every step (``assist_draft``); ``ngram`` and ``eos`` are unused."""
+        if not self._whole_model() or (assistant is not None and not assistant._whole_model()):
             raise NotImplementedError("prompt lookup decoding runs on a stage that holds the whole model")
+        if assistant is self:
+            raise ValueError("a stage cannot be its own assistant (the two would share one KV cache)")
+        if assistant is not None and assistant.device != self.device:
+            raise NotImplementedError(f"an assistant on {assistant.device} for a stage on {self.device}")
         if not 1 <= K <= nat.PL_MAX_DRAFT:
             raise ValueError(f"prompt lookup drafts 1..{nat.PL_MAX_DRAFT} tokens per step, got {K}")
+        # a captured assisted step holds its assistant's buffer addresses (its cache key holds the stage itself, so the
+        # addresses stay valid): keep the graphs of one assistant only
+        for key in [k for k in self.graphs if k[0] == "assist" and k[2] is not assistant]:
+            del self.graphs[key]
+        self.pl_assistant = assistant
+        if assistant is not None:
+            eos = ()                                 # an accepted EOS draft is cut on the host, as a decoded one
         dev, H, V, R = self.device, self.cfg.hidden, self.cfg.vocab, nat.VERIFY_MAX_ROWS
         if self.pl is None:
             self.pl = {"in_ids": torch.zeros(R, dtype=torch.int64, device=dev),       # last token + drafts (+ filler)
@@ -272,12 +293,16 @@ class CudaStage:
         self.pl_K = int(K)
 
     def _verify_body(self, draft: bool = True):
-        """draft -> embed K+1 ids -> layers -> final norm + lm_head + argmax of every row -> accept."""
+        """draft (n-gram kernel, or the assistant's K greedy tokens) -> embed K+1 ids -> layers -> final norm + lm_head +
+        argmax of every row -> accept."""
         pl, grp, cfg, v = self.pl, self.slots[0], self.cfg, self.params.v
         K = self.pl_K
         n = K + 1
         log, length, bits = self.hist_log[0, 0], self.hist_len[0, :1], self.hist_bits[0, 0]
-        if draft:
+        if draft and self.pl_assistant is not None:
+            self.pl_assistant.assist_draft(log, length, pl["in_ids"], K)
+            pl["n_cand"].fill_(K)
+        elif draft:
             nat.pl_draft(log, length, pl["params"], K, pl["in_ids"], pl["n_cand"])
         x, ids = pl["x"][:n], pl["ids"][:n]
         nat.embed_fwd(pl["in_ids"][:n], v["embed"], out=x)
@@ -297,12 +322,15 @@ class CudaStage:
         if not use_graph:
             self._verify_body()
             return
-        key = ("verify", self.pl_K + 1)
+        asst = self.pl_assistant
+        key = ("verify", self.pl_K + 1) if asst is None else ("assist", self.pl_K + 1, asst)
         g = self.graphs.get(key)
         if g is None:
             # warm up outside capture (first-use buffers, attributes), restoring what it touches
             grp, pl = self.slots[0], self.pl
             state = (grp.pos_dev, grp.kvlen_dev, pl["count"], pl["in_ids"], pl["n_cand"], self.hist_len, self.hist_bits)
+            if asst is not None:
+                state += (asst.slots[0].pos_dev, asst.slots[0].kvlen_dev)
             saved = [t.clone() for t in state]
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
@@ -340,6 +368,39 @@ class CudaStage:
         c0 = self.prompt_lookup_count()
         self._verify_body(draft=False)
         return self.prompt_lookup_tokens(c0, self.prompt_lookup_count()).tolist()
+
+    def verify_round(self) -> Tuple[List[int], List[int]]:
+        """One eager verify step with the run's own draft source (n-grams or the assistant).  Returns its drafts and
+        the tokens it emitted."""
+        c0 = self.prompt_lookup_count()
+        self._verify_body()
+        drafts = self.pl["in_ids"][1:1 + int(self.pl["n_cand"].item())].tolist()
+        return drafts, self.prompt_lookup_tokens(c0, self.prompt_lookup_count()).tolist()
+
+    # ------------------------------------------------------------------------------------------ assisted decoding
+    def assist_draft(self, log: torch.Tensor, length: torch.Tensor, in_ids: torch.Tensor, K: int):
+        """This stage as the assistant of another model's verify step (``prompt_lookup_begin(assistant=self)``): emit into
+        the current stream, graph-capturable, the greedy drafts in_ids[1..K] after the target's history (``log`` int32
+        [L], ``length`` int32 [1], on the target).  With P = length - 1, slot 0's cache must hold the history's keys up
+        to slot P-2 (the prompt's prefill, then earlier rounds).  The round rewrites slots P-1 and P from the history's
+        last two tokens as one 2-row verify step, whose last row gives in_ids[1], then feeds in_ids[i] at slot P+i for
+        i = 1..K-1 as decode steps, each giving in_ids[i+1].  Slots above P that hold rejected drafts are overwritten
+        by later rounds before they are read."""
+        grp, v = self.slots[0], self.params.v
+        if self.asst is None:
+            self.asst = {"in": torch.zeros(2, dtype=torch.int64, device=self.device),
+                         "x": torch.zeros(2, self.cfg.hidden, dtype=torch.bfloat16, device=self.device)}
+        a = self.asst
+        nat.assist_prep(log, length, a["in"], in_ids, grp.pos_dev, grp.kvlen_dev)      # pos = kv_len = P-1
+        nat.embed_fwd(a["in"], v["embed"], out=a["x"])
+        grp.verify_step_inplace(a["x"])
+        self._head_greedy(a["x"][1:], in_ids[1:2])
+        nat.advance_pos(grp.pos_dev, grp.kvlen_dev, 2)                                  # pos = kv_len = P+1
+        x = self.x_dec[0][:1]
+        for i in range(1, K):
+            nat.embed_fwd(in_ids[i:i + 1], v["embed"], out=x)
+            grp.decode_step_inplace(x)
+            self._head_greedy(x, in_ids[i + 1:i + 2])
 
     def check(self):
         for g in self.slots:

@@ -55,6 +55,7 @@ _SIGS = {
     "tl_prompt_lookup_draft": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "tl_prompt_lookup_accept": (c_int, [c_void_p] * 6 + [c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                                          c_void_p, c_int, c_void_p]),
+    "tl_assist_prep": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 5),
     "tl_rope_kv_fwd_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "tl_attn_prefill_fwd_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
@@ -532,6 +533,16 @@ def pl_accept(ids, in_ids, n_cand, log, length, bits, V: int, params, out_log, c
     _check(load().tl_prompt_lookup_accept(_p(ids), _p(in_ids), _p(n_cand), _p(log), _p(length), _p(bits), log.shape[-1], V,
                                           _p(params), _p(out_log), _p(count), out_log.numel(), _p(pos_dev), _p(kv_len_dev),
                                           K, _stream()), "tl_prompt_lookup_accept")
+
+
+def assist_prep(log, length, asst_in, in_ids, pos_dev, kv_len_dev):
+    """Row 0's history (log int32 [L], length int32 [1], L >= 2 tokens) -> the assistant's 2-row catch-up input
+    ``asst_in`` (the last two tokens) and positions (pos = kv_len = length - 2), and the target's in_ids[0]."""
+    require_device()
+    _i32(log, length, pos_dev, kv_len_dev)
+    assert asst_in.dtype == torch.int64 and in_ids.dtype == torch.int64 and asst_in.numel() >= 2 and in_ids.numel() >= 1
+    _check(load().tl_assist_prep(_p(log), _p(length), log.shape[-1], _p(asst_in), _p(in_ids), _p(pos_dev), _p(kv_len_dev),
+                                 _stream()), "tl_assist_prep")
 
 
 def advance_pos(pos_dev, kv_len_dev, delta: int):
