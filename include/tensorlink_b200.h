@@ -197,6 +197,19 @@ int tl_argmax_bf16(const void* logits, int64_t* ids_out, void* workspace, size_t
 size_t tl_sample_ws(int M);
 int tl_sample(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
               unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream);
+/* speculative sampling after a verify pass (Leviathan et al. Algorithm 1, HF _speculative_sampling), one row: the
+ * target's rows p_logits bf16 [K+1, V_p] and the assistant's q_logits bf16 [K, V_q], each warped by tl_sample's rules
+ * with the same temperature / top_k / top_p; the drafts d_i = in_ids[i+1] for i < n = min(*n_cand, K).  Draft i is kept
+ * while u_i * q_i(d_i) < p_i(d_i) (u_i: Philox row i); at the first rejection n the next token is drawn from
+ * norm((p_n - q_n)+) with d_n excluded (from p_n without d_n when that mass rounds to 0), else from p_n (Philox row 16).
+ * An id >= V_q has q = 0, a draft >= V_p has p = 0 (always rejected): exact over the union of the vocabularies.
+ * Output in tl_prompt_lookup_accept's form: ids_out[i] = in_ids[i+1] for i < n, ids_out[n] = the drawn token (never
+ * in_ids[n+1]); ids_out[n+1..K] are not written.  counter_dev: one int32 in device memory, advanced by one per call.
+ * workspace >= tl_spec_accept_ws(K) bytes.  Two launches: 2K+1 CTAs (one per row), then one CTA. */
+size_t tl_spec_accept_ws(int K);
+int tl_spec_accept(const void* p_logits, int V_p, const void* q_logits, int V_q, int K, const int64_t* in_ids,
+                   const int32_t* n_cand, float temperature, int top_k, float top_p, unsigned long long seed,
+                   int32_t* counter_dev, int64_t* ids_out, void* workspace, size_t ws_bytes, void* stream);
 
 /* ---- logits processors (csrc/logits_process.cu): HF's RepetitionPenaltyLogitsProcessor -> NoRepeatNGramLogitsProcessor
  * -> MinNewTokensLengthLogitsProcessor on the fp32 copy of the bf16 logits, before the argmax or the warpers above.

@@ -76,15 +76,19 @@ __device__ double block_excl_scan(double v, double* s_warp, double* total) {
     return before;
 }
 
-__global__ void __launch_bounds__(SM_THREADS) sample_kernel(const bf16* __restrict__ logits, int64_t* __restrict__ ids_out, int V,
-                                                            float inv_temp, int top_k, float top_p, unsigned long long seed,
-                                                            int32_t* __restrict__ counters, uint32_t* __restrict__ hist_all) {
-    const int row = blockIdx.x, tid = threadIdx.x;
-    const uint16_t* lr = reinterpret_cast<const uint16_t*>(logits) + (size_t)row * V;
-    uint32_t* hist = hist_all + (size_t)row * SM_BINS;
-    __shared__ double s_warp[32];
-    __shared__ int s_sel[4];
-    __shared__ double s_val[2];
+// The row analysis of the rules above: the histogram of the row's bf16 keys in ``hist`` (this row's SM_BINS bins in
+// global memory), then the max, the top-k key, the top-p key and the kept mass Z_kept of the bins.  Every kernel that
+// samples from a warped bf16 row (sample_kernel, spec_rows_kernel) calls this one function, so they keep the same
+// tokens with the same weights.  s_warp / s_sel / s_val: the CTA's shared scratch.
+struct RowStats {
+    float x_max;        // the max logit / temperature: weight(key) = __expf(key_value(key) * inv_temp - x_max)
+    int p_key;          // kept: key >= p_key
+    double Z_kept;      // the kept mass, summed over the bins
+};
+
+__device__ __forceinline__ RowStats row_analysis(const uint16_t* __restrict__ lr, int V, float inv_temp, int top_k, float top_p,
+                                                 uint32_t* __restrict__ hist, double* s_warp, int* s_sel, double* s_val) {
+    const int tid = threadIdx.x;
     for (int i = tid; i < SM_BINS; i += SM_THREADS) hist[i] = 0u;
     __syncthreads();
     for (int i = tid; i < V; i += SM_THREADS) atomicAdd(&hist[bf16_key(lr[i])], 1u);
@@ -151,6 +155,19 @@ __global__ void __launch_bounds__(SM_THREADS) sample_kernel(const bf16* __restri
         p_key = s_sel[2];
         Z_kept = s_val[0];
     }
+    return RowStats{x_max, p_key, Z_kept};
+}
+
+__global__ void __launch_bounds__(SM_THREADS) sample_kernel(const bf16* __restrict__ logits, int64_t* __restrict__ ids_out, int V,
+                                                            float inv_temp, int top_k, float top_p, unsigned long long seed,
+                                                            int32_t* __restrict__ counters, uint32_t* __restrict__ hist_all) {
+    const int row = blockIdx.x, tid = threadIdx.x;
+    const uint16_t* lr = reinterpret_cast<const uint16_t*>(logits) + (size_t)row * V;
+    __shared__ double s_warp[32];
+    __shared__ int s_sel[4];
+    __shared__ double s_val[2];
+    const auto [x_max, p_key, Z_kept] = row_analysis(lr, V, inv_temp, top_k, top_p, hist_all + (size_t)row * SM_BINS, s_warp,
+                                                     s_sel, s_val);
     // ---- draw and invert the CDF over the kept tokens in index order
     const uint32_t ctr = (uint32_t)counters[row];
     const double target = (double)philox_uniform(seed, (uint32_t)row, ctr) * Z_kept;
@@ -186,6 +203,121 @@ __global__ void __launch_bounds__(SM_THREADS) sample_kernel(const bf16* __restri
         }
         ids_out[row] = (int64_t)pick;
         counters[row] = (int32_t)(ctr + 1u);
+    }
+}
+
+// ================================================================================================ speculative sampling
+// Leviathan et al., Algorithm 1 (HF ``_speculative_sampling``) after a verify pass: the target's K+1 rows p_0..p_K and the
+// assistant's K rows q_0..q_{K-1}, each warped by the rules above (tl_sample's kept set and weights), drafts d_i =
+// in_ids[i+1] drawn from q_i.  Two launches:
+//   * spec_rows_kernel  one CTA per row (2K+1, in parallel): row_analysis -> SpecRow in the workspace
+//   * spec_draw_kernel  one CTA: draft i < n_cand is kept while u_i * q_i(d_i) < p_i(d_i) (u_i = Philox row i); at the
+//                       first rejection n the token is drawn from (p_n - q_n)+ without d_n, else from p_n (Philox row
+//                       SPEC_DRAW_ROW), by the inverse CDF in index order with fixed-order sums
+// Every probability is weight / Z_kept of its row, in double.  An id >= V_q has q = 0; a draft >= V_p has p = 0 and is
+// always rejected; ids >= V_p carry no residual mass, so the draw runs over 0..V_p-1.
+struct SpecRow {
+    float x_max;
+    int p_key;
+    double Z;
+};
+constexpr int SPEC_DRAW_ROW = 16;       // Philox row of the final draw; the acceptance uniforms take rows 0..K-1 (K <= 15)
+
+__device__ __forceinline__ double kept_weight(const uint16_t* lr, int t, const SpecRow& s, float inv_temp) {
+    const uint32_t key = bf16_key(lr[t]);
+    return (int)key >= s.p_key ? (double)__expf(key_value(key) * inv_temp - s.x_max) : 0.0;
+}
+
+__global__ void __launch_bounds__(SM_THREADS) spec_rows_kernel(const bf16* __restrict__ p_logits, int V_p,
+                                                               const bf16* __restrict__ q_logits, int V_q, int K, float inv_temp,
+                                                               int top_k, float top_p, SpecRow* __restrict__ rows,
+                                                               uint32_t* __restrict__ hist_all) {
+    const int r = blockIdx.x;                        // 0..K: p rows, K+1..2K: q rows
+    const bool is_p = r <= K;
+    const int V = is_p ? V_p : V_q;
+    const uint16_t* lr = reinterpret_cast<const uint16_t*>(is_p ? p_logits : q_logits) + (size_t)(is_p ? r : r - K - 1) * V;
+    __shared__ double s_warp[32];
+    __shared__ int s_sel[4];
+    __shared__ double s_val[2];
+    const RowStats rs = row_analysis(lr, V, inv_temp, top_k, top_p, hist_all + (size_t)r * SM_BINS, s_warp, s_sel, s_val);
+    if (threadIdx.x == 0) rows[r] = SpecRow{rs.x_max, rs.p_key, rs.Z_kept};
+}
+
+__global__ void __launch_bounds__(SM_THREADS) spec_draw_kernel(const bf16* __restrict__ p_logits, int V_p,
+                                                               const bf16* __restrict__ q_logits, int V_q, int K,
+                                                               const int64_t* __restrict__ in_ids, const int32_t* __restrict__ n_cand,
+                                                               float inv_temp, unsigned long long seed, int32_t* __restrict__ counter,
+                                                               const SpecRow* __restrict__ rows, int64_t* __restrict__ ids_out) {
+    const int tid = threadIdx.x;
+    const uint16_t* P = reinterpret_cast<const uint16_t*>(p_logits);
+    const uint16_t* Q = reinterpret_cast<const uint16_t*>(q_logits);
+    __shared__ double s_warp[32];
+    __shared__ int s_n, s_pick;
+    const uint32_t ctr = (uint32_t)*counter;
+    const int nc = max(0, min(*n_cand, K));
+    if (tid == 0) {
+        int n = 0;
+        for (; n < nc; ++n) {
+            const int64_t d = in_ids[n + 1];
+            const SpecRow &sp = rows[n], &sq = rows[K + 1 + n];
+            const double p = d >= 0 && d < V_p ? kept_weight(P + (size_t)n * V_p, (int)d, sp, inv_temp) / sp.Z : 0.0;
+            const double q = d >= 0 && d < V_q ? kept_weight(Q + (size_t)n * V_q, (int)d, sq, inv_temp) / sq.Z : 0.0;
+            // strict: u can be 0, and a token the target's warpers removed (p = 0) must never be kept
+            if (!((double)philox_uniform(seed, (uint32_t)n, ctr) * q < p)) break;
+        }
+        s_n = n;
+        s_pick = -1;
+    }
+    __syncthreads();
+    const int n = s_n;
+    const bool resid = n < nc;
+    const int64_t d = resid ? in_ids[n + 1] : -1;    // the rejected draft: never drawn, whatever the rounding
+    const uint16_t* pr = P + (size_t)n * V_p;
+    const uint16_t* qr = Q + (size_t)(resid ? n : 0) * V_q;
+    const SpecRow sp = rows[n], sq = rows[K + 1 + (resid ? n : 0)];
+    // resid: (p_n - q_n)+ in probabilities; otherwise p_n's kept weights (also the fallback when the residual mass is 0)
+    auto weight = [&](int t, bool res) -> double {
+        if (t == d) return 0.0;
+        const double wp = kept_weight(pr, t, sp, inv_temp);
+        if (!res) return wp;
+        const double wq = t < V_q ? kept_weight(qr, t, sq, inv_temp) / sq.Z : 0.0;
+        return fmax(0.0, wp / sp.Z - wq);
+    };
+    const double u = (double)philox_uniform(seed, (uint32_t)SPEC_DRAW_ROW, ctr);
+    const int per = (V_p + SM_THREADS - 1) / SM_THREADS;
+    const int i0 = tid * per, i1 = min(V_p, i0 + per);
+    bool res = resid;
+    double local_w, W, w_before;
+    for (;;) {
+        local_w = 0.0;
+        for (int i = i0; i < i1; ++i) local_w += weight(i, res);
+        w_before = block_excl_scan(local_w, s_warp, &W);
+        if (W > 0.0 || !res) break;
+        res = false;                                 // the residual rounded to 0 (p_n == q_n): draw from p_n
+    }
+    const double target = u * W;
+    if (local_w > 0.0 && w_before <= target && target < w_before + local_w) {
+        double c = w_before;
+        int pick = -1;
+        for (int i = i0; i < i1; ++i) {
+            const double w = weight(i, res);
+            if (w <= 0.0) continue;
+            pick = i;
+            c += w;
+            if (target < c) break;
+        }
+        s_pick = pick;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int pick = s_pick;
+        if (pick < 0) {                 // rounding left the target at / beyond the total: the last token of positive weight
+            for (int i = V_p - 1; i >= 0; --i)
+                if (weight(i, res) > 0.0) { pick = i; break; }
+        }
+        for (int i = 0; i < n; ++i) ids_out[i] = in_ids[i + 1];
+        ids_out[n] = (int64_t)pick;
+        *counter = (int32_t)(ctr + 1u);
     }
 }
 
@@ -404,6 +536,36 @@ int tl_sample(const void* logits, int64_t* ids_out, int M, int V, float temperat
     sample_kernel<<<M, SM_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, ids_out, V, 1.0f / temperature, top_k, top_p, seed,
                                                               counters_dev, (uint32_t*)workspace);
     return check_launch("tl_sample");
+}
+
+size_t tl_spec_accept_ws(int K) {
+    const size_t rows = (size_t)(K > 0 ? 2 * K + 1 : 0);
+    return rows * tl::SM_BINS * sizeof(uint32_t) + rows * sizeof(tl::SpecRow);
+}
+
+int tl_spec_accept(const void* p_logits, int V_p, const void* q_logits, int V_q, int K, const int64_t* in_ids,
+                   const int32_t* n_cand, float temperature, int top_k, float top_p, unsigned long long seed,
+                   int32_t* counter_dev, int64_t* ids_out, void* workspace, size_t ws_bytes, void* stream) {
+    using namespace tl;
+    TL_REQUIRE(p_logits && q_logits && in_ids && n_cand && counter_dev && ids_out && workspace, TL_ERR_INVALID,
+               "tl_spec_accept: null argument");
+    TL_REQUIRE(K >= 1 && K <= TL_PL_MAX_DRAFT && V_p >= 1 && V_q >= 1, TL_ERR_INVALID,
+               "tl_spec_accept: bad shape K=%d V_p=%d V_q=%d", K, V_p, V_q);
+    TL_REQUIRE(temperature > 0.f && top_p > 0.f && top_p <= 1.f && top_k >= 0, TL_ERR_INVALID,
+               "tl_spec_accept: temperature must be > 0, 0 < top_p <= 1, top_k >= 0 (got %g, %g, %d)", temperature, top_p, top_k);
+    TL_REQUIRE(ws_bytes >= tl_spec_accept_ws(K), TL_ERR_INVALID, "tl_spec_accept: workspace %zu < %zu", ws_bytes,
+               tl_spec_accept_ws(K));
+    cudaStream_t st = (cudaStream_t)stream;
+    uint32_t* hist = (uint32_t*)workspace;
+    SpecRow* rows = (SpecRow*)(hist + (size_t)(2 * K + 1) * SM_BINS);
+    const float inv_temp = 1.0f / temperature;
+    spec_rows_kernel<<<2 * K + 1, SM_THREADS, 0, st>>>((const bf16*)p_logits, V_p, (const bf16*)q_logits, V_q, K, inv_temp, top_k,
+                                                       top_p, rows, hist);
+    const int rc = check_launch("tl_spec_accept");
+    if (rc != TL_OK) return rc;
+    spec_draw_kernel<<<1, SM_THREADS, 0, st>>>((const bf16*)p_logits, V_p, (const bf16*)q_logits, V_q, K, in_ids, n_cand, inv_temp,
+                                               seed, counter_dev, rows, ids_out);
+    return check_launch("tl_spec_accept");
 }
 
 }  // extern "C"

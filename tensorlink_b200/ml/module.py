@@ -100,8 +100,8 @@ def _prompt_lookup(num_tokens, ngram, shape, max_new, max_seq, sampling=None, pr
     """HF's ``prompt_lookup_num_tokens`` / ``max_matching_ngram_size`` as {K, ngram}, or None when prompt lookup is off
     (``num_tokens`` None).  ``shape``: the [rows, S] of the prompt that reaches the cache.  Values HF rejects, more than
     PL_MAX_DRAFT drafts, more than one row, or a cache too short for the last verify step raise ValueError; what the
-    verify step does not implement (sampling, logits processors, several stages, another stage than the CUDA one,
-    more EOS ids than the device parameter block holds) raises NotImplementedError."""
+    verify step does not implement (logits processors, several stages, another stage than the CUDA one, more EOS ids
+    than the device parameter block holds) raises NotImplementedError.  ``sampling`` (do_sample) is accepted."""
     if num_tokens is None:
         return None
     n = 2 if ngram is None else ngram
@@ -117,8 +117,6 @@ def _prompt_lookup(num_tokens, ngram, shape, max_new, max_seq, sampling=None, pr
     if S + max_new + K > max_seq:
         raise ValueError(f"prompt lookup needs S + max_new_tokens + prompt_lookup_num_tokens <= max_seq (the last verify "
                          f"step writes K+1 cache slots); got {S} + {max_new} + {K} > {max_seq}")
-    if sampling is not None:
-        raise NotImplementedError("prompt_lookup_num_tokens with do_sample=True (drafts are verified greedily)")
     if procs is not None:
         raise NotImplementedError("prompt_lookup_num_tokens with repetition_penalty / no_repeat_ngram_size / min_new_tokens")
     if world > 1:
@@ -127,13 +125,15 @@ def _prompt_lookup(num_tokens, ngram, shape, max_new, max_seq, sampling=None, pr
         raise NotImplementedError(f"prompt_lookup_num_tokens with more than {PL_MAX_EOS} EOS ids")
     from .stage import CudaStage
     if not isinstance(stage, CudaStage):
-        raise NotImplementedError("prompt_lookup_num_tokens needs the CUDA stage")
+        raise NotImplementedError(f"prompt_lookup_num_tokens{' with do_sample=True' if sampling is not None else ''} needs "
+                                  "the CUDA stage")
     return {"K": K, "ngram": int(n)}
 
 
 # num_assistant_tokens when the keyword is absent: the K with the most expected tokens per ms in tools/bench_assisted.py
 # (Qwen2.5-7B target, Qwen2.5-0.5B assistant, one H100), with an ASSUMED agreement of 0.8 per draft token between the two
-# models.  It changes speed only, never the output.
+# models.  The same rule on sampled round costs (``--sampled``) also gives 2, so the default serves do_sample as well.  It
+# changes speed only: never the greedy output, nor the distribution of the sampled one.
 ASSISTED_DEFAULT_K = 2
 
 
@@ -146,9 +146,9 @@ def _device_key(d):
 def _assisted(target, assistant, num_tokens, shape, max_new, sampling=None, procs=None) -> dict:
     """HF's ``assistant_model`` / ``num_assistant_tokens`` as {K, ngram, assistant (its stage)}.  A non-DistributedModel
     raises TypeError; the target as its own assistant, a bad K (1..PL_MAX_DRAFT), more than one row or a cache of either
-    model too short for the last verify step raise ValueError; what the verify step does not implement (sampling,
-    logits processors, several stages on either side, a stage other than the CUDA one, an assistant on another device)
-    raises NotImplementedError."""
+    model too short for the last verify step raise ValueError; what the verify step does not implement (logits
+    processors, several stages on either side, a stage other than the CUDA one, an assistant on another device) raises
+    NotImplementedError.  ``sampling`` (do_sample) is accepted."""
     if not isinstance(assistant, DistributedModel):
         raise TypeError(f"assistant_model has to be a DistributedModel, got {type(assistant).__name__}; wrap an HF "
                         "module as DistributedModel(hf_model, training=False)")
@@ -166,15 +166,14 @@ def _assisted(target, assistant, num_tokens, shape, max_new, sampling=None, proc
         if S + max_new + K > m.max_seq:
             raise ValueError(f"assisted decoding needs S + max_new_tokens + num_assistant_tokens <= max_seq of {who} (the "
                              f"last verify step writes K+1 cache slots); got {S} + {max_new} + {K} > {m.max_seq}")
-    if sampling is not None:
-        raise NotImplementedError("assistant_model with do_sample=True (drafts are verified greedily)")
     if procs is not None:
         raise NotImplementedError("assistant_model with repetition_penalty / no_repeat_ngram_size / min_new_tokens")
     if target.world > 1 or assistant.world > 1:
         raise NotImplementedError("assistant_model with a model or an assistant on a pipeline of more than one stage")
     from .stage import CudaStage
     if not isinstance(target.stage, CudaStage) or not isinstance(assistant.stage, CudaStage):
-        raise NotImplementedError("assistant_model needs the CUDA stage on the model and on the assistant")
+        raise NotImplementedError(f"assistant_model{' with do_sample=True' if sampling is not None else ''} needs the CUDA "
+                                  "stage on the model and on the assistant")
     if _device_key(assistant.stage.device) != _device_key(target.stage.device):
         raise NotImplementedError(f"assistant_model on {assistant.stage.device} for a model on {target.stage.device} "
                                   "(both run on one device)")
@@ -561,17 +560,19 @@ class DistributedModel(torch.nn.Module):
             self.link.broadcast(out, 0)              # every rank returns the whole result, prompt and pads included
         return out
 
-    def _generate_lookup(self, input_ids, max_new, streamer, use_graph, lookup):
-        """Greedy generation of one row with prompt-lookup drafts (``_prompt_lookup``) or an assistant's (``_assisted``)
-        on the one CUDA stage: prefill, the first token from the head, then verify steps (ml/stage.py
-        ``prompt_lookup_step``), each drafting K tokens on the device (from the row's history, or by the assistant,
+    def _generate_lookup(self, input_ids, max_new, streamer, use_graph, lookup, sampling):
+        """Generation of one row with prompt-lookup drafts (``_prompt_lookup``) or an assistant's (``_assisted``) on the
+        one CUDA stage, greedy or sampled (``sampling``): prefill, the first token from the head, then verify steps
+        (ml/stage.py ``prompt_lookup_step``), each drafting K tokens on the device (from the row's history, or by the assistant,
         whose cache starts with the prompt's prefill) and emitting 1..K+1 tokens.  The host replays rounds of
         r = max(1, (max_new - count) // (K+1)) steps (at most EOS_CHECK_EVERY with ``eos_token_id``), so no step runs
         once max_new tokens are out, and reads the token count once per round."""
         st, dev = self.stage, self.device
         K, asst = lookup["K"], lookup.get("assistant")
         S = input_ids.shape[1]
-        st.set_sampling(None)                      # greedy, no logits processors: the plain argmax head
+        st.set_sampling(sampling)                  # no logits processors: the plain argmax or sampling head
+        if sampling is not None:
+            st.sample_ctr.zero_()                  # a seed names ONE set of streams (ml/stage.py STREAM_PL_ROWS)
         st.set_logits_processors(None)
         t0 = time.perf_counter()
         ids = input_ids.to(dev)
@@ -627,19 +628,27 @@ class DistributedModel(torch.nn.Module):
         With ``do_sample`` a padded batch draws one stream per micro-batch slot, exactly as an unpadded batch does, so
         a row's tokens depend on the seed and its place in the batch, not on its prompt length.
         ``prompt_lookup_num_tokens=K`` (1..15; ``max_matching_ngram_size`` n, default 2): HF's prompt-lookup decoding for
-        one greedy row on one stage.  Each step drafts up to K tokens that followed an earlier occurrence of the last
+        one row on one stage.  Each step drafts up to K tokens that followed an earlier occurrence of the last
         n-gram and verifies them with the current token as K+1 rows in one pass over the weights (csrc/prompt_lookup.cu);
-        the output is greedy decoding's.  ``self.timers["prompt_lookup_steps"]`` counts the verify steps.
+        greedy, the output is greedy decoding's.  With ``do_sample`` every row draws a token from the model's warped
+        distribution, and the drafts those draws agree with are kept with the draw that follows them, as in HF.
+        ``self.timers["prompt_lookup_steps"]`` counts the verify steps.
         ``assistant_model=draft`` (another ``DistributedModel`` on this device, one stage; wrap an HF module as
-        ``DistributedModel(hf_model, training=False)``), ``num_assistant_tokens=K`` (1..15): HF's assisted decoding with
-        greedy selection, for one greedy row on one stage.  Each step the assistant greedily drafts K tokens and the model
-        verifies them with its current token as K+1 rows in one pass over its weights, keeping the agreeing prefix and
-        its own next token, all on the GPU; the output is greedy decoding's.  The two models may differ in every
-        dimension, the vocabulary included: an id one of them cannot embed reads its embedding row 0, which can only
-        cost acceptance, since a draft is kept only where it equals the model's own argmax.  Matching tokenizers are the
+        ``DistributedModel(hf_model, training=False)``), ``num_assistant_tokens=K`` (1..15): HF's assisted decoding for
+        one row on one stage.  Each step the assistant drafts K tokens and the model verifies them with its current
+        token as K+1 rows in one pass over its weights, keeping the agreeing prefix and its own next token, all on the
+        GPU; greedy, the output is greedy decoding's.  With ``do_sample`` the assistant samples each draft from its own
+        distribution warped by the same ``temperature`` / ``top_k`` / ``top_p``, and the model keeps it by speculative
+        sampling (Leviathan et al.; csrc/sample.cu ``tl_spec_accept``).  Sampled with either draft source, every emitted
+        token follows the model's warped distribution, as plain sampling's does, and a seed reproduces its tokens; they
+        are other draws than plain sampling's for that seed (the streams: ml/stage.py STREAM_PL_ROWS).  The two models may differ in
+        every dimension, the vocabulary included: an id one of them cannot embed reads its embedding row 0, which can
+        only cost acceptance; sampled, an id outside the assistant's vocabulary has q = 0 and a draft outside the model's
+        has p = 0 (rejected), which extends HF's rule, defined for equal vocabularies only.  Matching tokenizers are the
         caller's responsibility, as in HF.  Without ``num_assistant_tokens`` K is ASSISTED_DEFAULT_K, the K with the
         most expected tokens per ms on an H100 for a Qwen2.5-7B model and a Qwen2.5-0.5B assistant ASSUMING an
-        agreement of 0.8 per draft token (not measured on real checkpoints); it changes speed only, never the output.
+        agreement of 0.8 per draft token (not measured on real checkpoints); it changes speed only: never the greedy output,
+        nor the distribution of the sampled one.
         ``num_assistant_tokens_schedule`` may only be "constant" and ``assistant_confidence_threshold`` only None.
         ``self.timers["assisted_steps"]`` counts the verify steps."""
         input_ids = kwargs.pop("input_ids", args[0] if args else None)
@@ -687,7 +696,7 @@ class DistributedModel(torch.nn.Module):
             lookup = _prompt_lookup(lookup, ngram, tuple(input_ids.shape) if input_ids is not None else (1, 0), max_new,
                                     self.max_seq, sampling, procs, self.world, st, self._eos[0])
         if lookup is not None:
-            result = self._generate_lookup(input_ids, max_new, streamer, use_graph, lookup)
+            result = self._generate_lookup(input_ids, max_new, streamer, use_graph, lookup, sampling)
             if padded is not None and padded[0].shape[1]:
                 result = torch.cat([padded[0].to(result.device), result], dim=1)
             return result

@@ -15,6 +15,21 @@ from .. import native as nat
 from .configs import ShardModelConfig
 from .shard import CudaLayerGroup, ShardParams, gemv_max_rows
 
+# Philox streams of one sampled generate call, all keyed by its ``seed``: stream s draws with the key seed + GOLDEN * s
+# (mod 2^64).  The plain head sampler of slot m is stream m (so the first token of a drafted run is slot 0's); the
+# drafted verify steps take the streams below, which no slot index reaches.  GOLDEN is odd, so distinct streams have
+# distinct keys.  Within a stream a (Philox row, counter) pair is used once:
+#   STREAM_PL_ROWS   prompt lookup: row i of the K+1 verify rows draws on Philox row i, counter pl["ctr"][i]
+#   STREAM_DRAFTS    the assistant's drafts: Philox row 0, counter pl["ctr"][16], one step per draft
+#   STREAM_ACCEPT    tl_spec_accept: u_i on Philox row i, the final draw on row 16, counter pl["ctr"][17], one step a round
+GOLDEN = 0x9E3779B97F4A7C15
+STREAM_PL_ROWS, STREAM_DRAFTS, STREAM_ACCEPT = 2 ** 32 - 1, 2 ** 32 - 2, 2 ** 32 - 3
+CTR_DRAFTS, CTR_ACCEPT = nat.VERIFY_MAX_ROWS, nat.VERIFY_MAX_ROWS + 1
+
+
+def stream_seed(seed: int, stream: int) -> int:
+    return (seed + GOLDEN * stream) & (2 ** 64 - 1)
+
 
 class CudaStage:
     def __init__(self, cfg: ShardModelConfig, layer_ids, has_embed: bool, has_head: bool, device,
@@ -252,7 +267,11 @@ class CudaStage:
         the history (largest n-gram ``ngram``, EOS ids ``eos``) and runs K+1 rows; the history never grows past
         ``max_length`` (prompt + max_new_tokens).
         ``assistant``: assisted decoding instead.  That stage (another model on this device, its slot 0 prefilled with
-        the prompt) drafts K tokens greedily in every step (``assist_draft``); ``ngram`` and ``eos`` are unused."""
+        the prompt) drafts K tokens greedily in every step (``assist_draft``); ``ngram`` and ``eos`` are unused.
+        After ``set_sampling`` the steps sample: prompt lookup draws every verify row from its warped distribution and
+        keeps the drafts the draws agree with (HF's sampled candidate check); an assistant samples its drafts and the
+        step keeps them by speculative sampling (``tl_spec_accept``).  The streams are described at STREAM_PL_ROWS;
+        their counters restart at 0 here."""
         if not self._whole_model() or (assistant is not None and not assistant._whole_model()):
             raise NotImplementedError("prompt lookup decoding runs on a stage that holds the whole model")
         if assistant is self:
@@ -281,6 +300,12 @@ class CudaStage:
                        "head_ws": torch.empty(max(nat.lmhead_ws(8, V), R * 64 * 8 + 256), dtype=torch.uint8, device=dev),
                        "out_log": torch.zeros(0, dtype=torch.int64, device=dev)}
         pl = self.pl
+        if self.sampling is not None and "ctr" not in pl:
+            pl["ctr"] = torch.zeros(R + 2, dtype=torch.int32, device=dev)        # see STREAM_PL_ROWS
+            pl["sample_ws"] = torch.empty(nat.sample_ws(R), dtype=torch.uint8, device=dev)
+            pl["spec_ws"] = torch.empty(nat.spec_accept_ws(nat.PL_MAX_DRAFT), dtype=torch.uint8, device=dev)
+        if "ctr" in pl:
+            pl["ctr"].zero_()
         S = seq.shape[1] - 1
         if pl["out_log"].numel() < max_length - S:
             pl["out_log"] = torch.zeros(max(max_length - S, 64), dtype=torch.int64, device=dev)
@@ -293,21 +318,36 @@ class CudaStage:
         self.pl_K = int(K)
 
     def _verify_body(self, draft: bool = True):
-        """draft (n-gram kernel, or the assistant's K greedy tokens) -> embed K+1 ids -> layers -> final norm + lm_head +
-        argmax of every row -> accept."""
+        """draft (n-gram kernel, or the assistant's K tokens) -> embed K+1 ids -> layers -> final norm + lm_head + argmax
+        of every row -> accept.  Sampled (``set_sampling``): the lm_head writes the K+1 logits rows, then one draw per row
+        (prompt lookup) or speculative sampling against the assistant's rows, then the same accept."""
         pl, grp, cfg, v = self.pl, self.slots[0], self.cfg, self.params.v
         K = self.pl_K
         n = K + 1
+        s, asst = self.sampling, self.pl_assistant
         log, length, bits = self.hist_log[0, 0], self.hist_len[0, :1], self.hist_bits[0, 0]
-        if draft and self.pl_assistant is not None:
-            self.pl_assistant.assist_draft(log, length, pl["in_ids"], K)
+        if draft and asst is not None:
+            asst.assist_draft(log, length, pl["in_ids"], K, None if s is None else (s, pl["ctr"][CTR_DRAFTS:CTR_DRAFTS + 1]))
             pl["n_cand"].fill_(K)
         elif draft:
             nat.pl_draft(log, length, pl["params"], K, pl["in_ids"], pl["n_cand"])
         x, ids = pl["x"][:n], pl["ids"][:n]
         nat.embed_fwd(pl["in_ids"][:n], v["embed"], out=x)
         grp.verify_step_inplace(x)
-        if n <= gemv_max_rows():
+        if s is not None:
+            logits = pl["logits"][:n]
+            if n <= gemv_max_rows():
+                nat.gemv(x, v["head"], out=logits, norm_w=v["norm"], eps=cfg.rms_eps, counter=self.head_ctr)
+            else:
+                nat.rmsnorm_fwd(x, v["norm"], cfg.rms_eps, out=pl["hn"][:n])
+                nat.gemm(pl["hn"][:n], v["head"], out=logits)
+            warp = (s["temperature"], s["top_k"], s["top_p"])
+            if asst is None:
+                nat.sample(logits, ids, pl["ctr"][:n], pl["sample_ws"], *warp, stream_seed(s["seed"], STREAM_PL_ROWS))
+            else:
+                nat.spec_accept(logits, asst.asst["q"][:K], pl["in_ids"], pl["n_cand"], pl["ctr"][CTR_ACCEPT:CTR_ACCEPT + 1],
+                                ids, pl["spec_ws"], *warp, stream_seed(s["seed"], STREAM_ACCEPT))
+        elif n <= gemv_max_rows():
             nat.lmhead_argmax(x, v["head"], v["norm"], cfg.rms_eps, ids, pl["logits"][:n], pl["head_ws"], self.head_ctr)
         else:
             nat.rmsnorm_fwd(x, v["norm"], cfg.rms_eps, out=pl["hn"][:n])
@@ -322,8 +362,8 @@ class CudaStage:
         if not use_graph:
             self._verify_body()
             return
-        asst = self.pl_assistant
-        key = ("verify", self.pl_K + 1) if asst is None else ("assist", self.pl_K + 1, asst)
+        asst, sampled = self.pl_assistant, self.sampling is not None
+        key = ("verify", self.pl_K + 1, sampled) if asst is None else ("assist", self.pl_K + 1, asst, sampled)
         g = self.graphs.get(key)
         if g is None:
             # warm up outside capture (first-use buffers, attributes), restoring what it touches
@@ -331,6 +371,8 @@ class CudaStage:
             state = (grp.pos_dev, grp.kvlen_dev, pl["count"], pl["in_ids"], pl["n_cand"], self.hist_len, self.hist_bits)
             if asst is not None:
                 state += (asst.slots[0].pos_dev, asst.slots[0].kvlen_dev)
+            if sampled:
+                state += (pl["ctr"],)                # the warm-up step must not consume a draw
             saved = [t.clone() for t in state]
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
@@ -371,36 +413,54 @@ class CudaStage:
 
     def verify_round(self) -> Tuple[List[int], List[int]]:
         """One eager verify step with the run's own draft source (n-grams or the assistant).  Returns its drafts and
-        the tokens it emitted."""
+        the tokens it emitted.  A sampled step leaves what its draws read: the counters ``pl["ctr"]``, the target's rows
+        ``pl["logits"][:K+1]`` and the assistant's rows ``asst["q"][:K]``."""
         c0 = self.prompt_lookup_count()
         self._verify_body()
         drafts = self.pl["in_ids"][1:1 + int(self.pl["n_cand"].item())].tolist()
         return drafts, self.prompt_lookup_tokens(c0, self.prompt_lookup_count()).tolist()
 
     # ------------------------------------------------------------------------------------------ assisted decoding
-    def assist_draft(self, log: torch.Tensor, length: torch.Tensor, in_ids: torch.Tensor, K: int):
+    def assist_draft(self, log: torch.Tensor, length: torch.Tensor, in_ids: torch.Tensor, K: int,
+                     sample: Optional[tuple] = None):
         """This stage as the assistant of another model's verify step (``prompt_lookup_begin(assistant=self)``): emit into
         the current stream, graph-capturable, the greedy drafts in_ids[1..K] after the target's history (``log`` int32
         [L], ``length`` int32 [1], on the target).  With P = length - 1, slot 0's cache must hold the history's keys up
         to slot P-2 (the prompt's prefill, then earlier rounds).  The round rewrites slots P-1 and P from the history's
         last two tokens as one 2-row verify step, whose last row gives in_ids[1], then feeds in_ids[i] at slot P+i for
         i = 1..K-1 as decode steps, each giving in_ids[i+1].  Slots above P that hold rejected drafts are overwritten
-        by later rounds before they are read."""
-        grp, v = self.slots[0], self.params.v
+        by later rounds before they are read.
+        ``sample`` = (sampling dict, counter int32[1]): draft i is drawn instead from this model's warped row (the
+        target's temperature / top_k / top_p, stream STREAM_DRAFTS), which stays in ``asst["q"][i]`` for the target's
+        speculative sampling."""
+        grp, v, dev = self.slots[0], self.params.v, self.device
         if self.asst is None:
-            self.asst = {"in": torch.zeros(2, dtype=torch.int64, device=self.device),
-                         "x": torch.zeros(2, self.cfg.hidden, dtype=torch.bfloat16, device=self.device)}
+            self.asst = {"in": torch.zeros(2, dtype=torch.int64, device=dev),
+                         "x": torch.zeros(2, self.cfg.hidden, dtype=torch.bfloat16, device=dev)}
         a = self.asst
+        if sample is not None and "q" not in a:
+            a["q"] = torch.zeros(nat.PL_MAX_DRAFT, self.cfg.vocab, dtype=torch.bfloat16, device=dev)
+            a["ws"] = torch.empty(nat.sample_ws(1), dtype=torch.uint8, device=dev)
+
+        def head(h, out, i):
+            if sample is None:
+                self._head_greedy(h, out)
+                return
+            s, ctr = sample
+            q = a["q"][i:i + 1]
+            nat.gemv(h, v["head"], out=q, norm_w=v["norm"], eps=self.cfg.rms_eps, counter=self.head_ctr)
+            nat.sample(q, out, ctr, a["ws"], s["temperature"], s["top_k"], s["top_p"], stream_seed(s["seed"], STREAM_DRAFTS))
+
         nat.assist_prep(log, length, a["in"], in_ids, grp.pos_dev, grp.kvlen_dev)      # pos = kv_len = P-1
         nat.embed_fwd(a["in"], v["embed"], out=a["x"])
         grp.verify_step_inplace(a["x"])
-        self._head_greedy(a["x"][1:], in_ids[1:2])
+        head(a["x"][1:], in_ids[1:2], 0)
         nat.advance_pos(grp.pos_dev, grp.kvlen_dev, 2)                                  # pos = kv_len = P+1
         x = self.x_dec[0][:1]
         for i in range(1, K):
             nat.embed_fwd(in_ids[i:i + 1], v["embed"], out=x)
             grp.decode_step_inplace(x)
-            self._head_greedy(x, in_ids[i + 1:i + 2])
+            head(x, in_ids[i + 1:i + 2], i)
 
     def check(self):
         for g in self.slots:

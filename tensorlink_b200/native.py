@@ -81,6 +81,9 @@ _SIGS = {
     "tl_sample_ws": (c_size_t, [c_int]),
     "tl_sample": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p, c_void_p, c_size_t,
                           c_void_p]),
+    "tl_spec_accept_ws": (c_size_t, [c_int]),
+    "tl_spec_accept": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_float,
+                               ctypes.c_uint64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "tl_logits_proc_ws": (c_size_t, [c_int, c_int]),
     "tl_history_fill": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "tl_argmax_proc": (c_int, [c_void_p] * 6 + [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
@@ -426,6 +429,27 @@ def sample(logits, ids_out, counters, ws, temperature: float = 1.0, top_k: int =
     assert ids_out.dtype == torch.int64 and counters.dtype == torch.int32 and counters.numel() >= M
     _check(load().tl_sample(_p(logits), _p(ids_out), M, V, float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1),
                             _p(counters), _p(ws), ws.numel() * ws.element_size(), _stream()), "tl_sample")
+
+
+def spec_accept_ws(K: int) -> int:
+    return int(load().tl_spec_accept_ws(K))
+
+
+def spec_accept(p_logits, q_logits, in_ids, n_cand, counter, ids_out, ws, temperature: float = 1.0, top_k: int = 0,
+                top_p: float = 1.0, seed: int = 0):
+    """Speculative sampling of one verify step: the target's rows p_logits [K+1, V_p], the assistant's q_logits [K, V_q]
+    (both bf16), the drafts in_ids[1..n_cand] drawn from q -> ids_out[0..n] in ``pl_accept``'s form (the kept drafts,
+    then the drawn token); ``counter`` int32[1] advances by one per call."""
+    require_device()
+    _bf16(p_logits, q_logits)
+    K = q_logits.shape[0]
+    if p_logits.shape[0] != K + 1:
+        raise NativeError(f"spec_accept: {p_logits.shape[0]} target rows for {K} assistant rows (K+1 expected)")
+    _i32(n_cand, counter)
+    assert in_ids.dtype == torch.int64 and ids_out.dtype == torch.int64 and in_ids.numel() >= K + 1 and ids_out.numel() >= K + 1
+    _check(load().tl_spec_accept(_p(p_logits), p_logits.shape[1], _p(q_logits), q_logits.shape[1], K, _p(in_ids), _p(n_cand),
+                                 float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1), _p(counter),
+                                 _p(ids_out), _p(ws), ws.numel() * ws.element_size(), _stream()), "tl_spec_accept")
 
 
 LP_PENALTY, LP_NGRAM, LP_MIN_NEW, LP_PROMPT, LP_N_EOS, LP_EOS, LP_MAX_EOS = 0, 1, 2, 3, 4, 5, 8

@@ -9,7 +9,10 @@
     position where the two outputs differ, if they do (with synthetic weights many top-2 margins are below bf16
     resolution, so the two greedy runs may fork there).
 
-    python tools/bench_prompt_lookup.py [--model Qwen/Qwen2.5-7B] [--rounds 5] [--out FILE]
+With ``--sampled`` every variant samples at HF's defaults (temperature 1, top_k 50, SAMPLING): the decode step draws
+its token and the verify step draws one token per row; the end-to-end runs use one fixed seed.
+
+    python tools/bench_prompt_lookup.py [--model Qwen/Qwen2.5-7B] [--rounds 5] [--sampled] [--out FILE]
 
 Prints one JSON line, with the card's name, power limit and max SM clock read in the same run.
 """
@@ -28,6 +31,7 @@ import torch  # noqa: E402
 Q_LENS = (2, 3, 4, 8, 11, 16)
 STEPS = 32
 PROMPT = 128
+SAMPLING = {"temperature": 1.0, "top_k": 50, "top_p": 1.0, "seed": 1234}
 
 
 def _card():
@@ -44,7 +48,7 @@ def _spread(ts):
     return {"median": round(statistics.median(ts), 4), "min": round(min(ts), 4), "max": round(max(ts), 4)}
 
 
-def step_costs(model, rounds):
+def step_costs(model, rounds, sampled=False):
     """(a): ms per graph replay of the plain decode step and of the verify step at each q_len."""
     from tensorlink_b200.ml import DistributedModel
     from tensorlink_b200.ml.weights import synthetic_tokens
@@ -52,7 +56,7 @@ def step_costs(model, rounds):
     st, cfg = dm.stage, dm.cfg
     grp = st.slots[0]
     ids = synthetic_tokens(cfg, 1, PROMPT).cuda()
-    st.set_sampling(None)
+    st.set_sampling(SAMPLING if sampled else None)
     st.set_logits_processors(None)
     x = st.prefill(st.embed(ids), 0, 0)
     first = st.ids_dec[0][:1]
@@ -101,15 +105,16 @@ def step_costs(model, rounds):
     return res
 
 
-def end_to_end(model, rounds, K, new, period=32, times=4):
+def end_to_end(model, rounds, K, new, period=32, times=4, sampled=False):
     """(b): tokens per second with and without prompt_lookup_num_tokens=K after a self-repeating prompt."""
     from tensorlink_b200.ml import DistributedModel
     from tensorlink_b200.ml.weights import synthetic_tokens
     cfg_prompt = period * times
     dm = DistributedModel(model, training=False, max_batch=1, max_seq=cfg_prompt + new + K + 8, init="device")
     ids = synthetic_tokens(dm.cfg, 1, period).repeat(1, times)
-    runs = {"plain": lambda: dm.generate(ids, max_new_tokens=new),
-            "lookup": lambda: dm.generate(ids, max_new_tokens=new, prompt_lookup_num_tokens=K)}
+    kw = dict(do_sample=True, **SAMPLING) if sampled else {}
+    runs = {"plain": lambda: dm.generate(ids, max_new_tokens=new, **kw),
+            "lookup": lambda: dm.generate(ids, max_new_tokens=new, prompt_lookup_num_tokens=K, **kw)}
     outs = {k: fn().cpu() for k, fn in runs.items()}    # warm-up (graph capture) and the outputs compared below
     times_s = {k: [] for k in runs}
     steps = None
@@ -140,11 +145,13 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--k", type=int, default=10)
     ap.add_argument("--new", type=int, default=256)
+    ap.add_argument("--sampled", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    res = {"model": a.model, **_card(), "batch": 1, "prompt_a": PROMPT, "steps_per_round": STEPS, "rounds": a.rounds}
-    res["step_cost"] = step_costs(a.model, a.rounds)
-    res["end_to_end"] = end_to_end(a.model, a.rounds, a.k, a.new)
+    res = {"model": a.model, **_card(), "batch": 1, "prompt_a": PROMPT, "steps_per_round": STEPS, "rounds": a.rounds,
+           "sampling": SAMPLING if a.sampled else None}
+    res["step_cost"] = step_costs(a.model, a.rounds, a.sampled)
+    res["end_to_end"] = end_to_end(a.model, a.rounds, a.k, a.new, sampled=a.sampled)
     line = json.dumps(res)
     print(line, flush=True)
     if a.out:
