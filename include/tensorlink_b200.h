@@ -103,6 +103,21 @@ int tl_gemv_bf16_ctr(const void* x, const void* W, void* y, int M, int N, int K,
                      const void* residual, const void* norm_w, float eps, int flags, unsigned* counter,
                      const void* next_W, size_t next_bytes, void* stream);
 
+/* ---- FP8 weights (HF's fine-grained FP8 checkpoints, weight-only): W[N,K] float8_e4m3fn with fp32 scales[N][K/128],
+ * one per row and 128-column group (HF's weight_scale_inv of the row's 128x128 block).  The weight used is
+ * bf16(float(W[n,k]) * scales[n][k/128]), the bf16 weight of HF's dequantized checkpoint.
+ * tl_gemv_fp8 / tl_gemv_fp8_ctr: tl_gemv_bf16 / tl_gemv_bf16_ctr over that weight (same flags, counter block and
+ * prefetch hint; next_bytes counts bytes of whatever the next launch streams).  The result equals tl_gemv_bf16's over
+ * the dequantized matrix bit for bit.  Needs K % 128 == 0 and a 16-byte aligned W.
+ * tl_dequant_fp8: out[N,K] bf16 = that weight, for the GEMM paths (prefill, batched decode); HBM-bound. */
+#define TL_FP8_BLOCK 128
+int tl_gemv_fp8(const void* x, const void* W, const float* scales, void* y, int M, int N, int K, const void* bias,
+                const void* residual, const void* norm_w, float eps, int flags, void* stream);
+int tl_gemv_fp8_ctr(const void* x, const void* W, const float* scales, void* y, int M, int N, int K, const void* bias,
+                    const void* residual, const void* norm_w, float eps, int flags, unsigned* counter,
+                    const void* next_W, size_t next_bytes, void* stream);
+int tl_dequant_fp8(const void* W, const float* scales, void* out, int N, int K, void* stream);
+
 /* ---- K3  rotary tables (modeling_qwen2.py:102-113): cos/sin[pos, d/2] = bf16(cos/sin(pos * inv_freq)) */
 int tl_rope_table(const float* inv_freq, void* cos_tab, void* sin_tab, int max_pos, int half_dim, void* stream);
 

@@ -12,7 +12,7 @@ pids=()
 for s in "${srcs[@]}"; do
   o="$objdir/$(basename "${s%.cu}").o"
   objs+=("$o")
-  if [[ ! -f "$o" || "$s" -nt "$o" || "${BASH_SOURCE[0]}" -nt "$o" || "$here/common.cuh" -nt "$o" || "$here/gemm_common.cuh" -nt "$o" || "$here/../../include/tensorlink_b200.h" -nt "$o" ]]; then
+  if [[ ! -f "$o" || "$s" -nt "$o" || "${BASH_SOURCE[0]}" -nt "$o" || "$here/common.cuh" -nt "$o" || "$here/gemm_common.cuh" -nt "$o" || "$here/fp8.cuh" -nt "$o" || "$here/../../include/tensorlink_b200.h" -nt "$o" ]]; then
     nvcc -gencode arch=compute_90a,code=$arch -O3 -std=c++17 -lineinfo -Xcompiler -fPIC \
          ${TL_NVCC_EXTRA:-} -c "$s" -o "$o" &
     pids+=($!)

@@ -10,18 +10,22 @@
 #include <mutex>
 
 #include "common.cuh"
+#include "fp8.cuh"
 
 namespace tl {
 
 constexpr int GEMV_THREADS = 256;
 constexpr int GEMV_WARPS = GEMV_THREADS / 32;
 
-template <int M, int G, int WPI>
-__global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W,
-                                                            bf16* __restrict__ y, int N, int K,
-                                                            const bf16* __restrict__ bias,
-                                                            const bf16* __restrict__ residual,
-                                                            const bf16* __restrict__ norm_w, float eps, int flags) {
+// The body of both kernels below.  WT: bf16, or fp8_e4m3 with `scales` [N][K/128]: each lane forms bf16(float(w) *
+// scale) from an 8-byte vector at the bf16 kernel's vector index, so the FMA sequence of every output is the bf16
+// kernel's over the dequantized matrix.
+template <typename WT, int M, int G, int WPI>
+__device__ __forceinline__ void gemv_body(const bf16* __restrict__ x, const WT* __restrict__ W, bf16* __restrict__ y,
+                                          int N, int K, const bf16* __restrict__ bias, const bf16* __restrict__ residual,
+                                          const bf16* __restrict__ norm_w, float eps, int flags,
+                                          const float* __restrict__ scales) {
+    constexpr bool FP8 = sizeof(WT) == 1;
     constexpr int SLOTS = GEMV_WARPS / WPI;
     constexpr int ROWS = 2 * G;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -98,18 +102,26 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const bf16* __restri
             for (int m = 0; m < M; ++m) acc[r][m] = 0.f;
         if (item < n_items) {
             const int row0 = item * ROWS;
-            const uint4* wrow[ROWS];
+            const WT* wrow[ROWS];
+            const float* srow[ROWS];
 #pragma unroll
             for (int r = 0; r < ROWS; ++r) {
                 int row = row0 + r;
                 if (row >= N) row = N - 1;   // clamp (result discarded)
-                wrow[r] = reinterpret_cast<const uint4*>(W + (size_t)row * K);
+                wrow[r] = W + (size_t)row * K;
+                if constexpr (FP8) srow[r] = scales + (size_t)row * (K / TL_FP8_BLOCK);
             }
 #pragma unroll 2
             for (int v = wi * 32 + lane; v < nvec; v += WPI * 32) {
                 uint4 wv[ROWS];
+                float wf[FP8 ? ROWS : 1][8];
 #pragma unroll
-                for (int r = 0; r < ROWS; ++r) wv[r] = ldg_nc_v4(wrow[r] + v);
+                for (int r = 0; r < ROWS; ++r) {
+                    if constexpr (FP8)
+                        fp8x8_scaled(__ldg(reinterpret_cast<const uint2*>(wrow[r]) + v), __ldg(srow[r] + (v >> 4)), wf[r]);
+                    else
+                        wv[r] = ldg_nc_v4(reinterpret_cast<const uint4*>(wrow[r]) + v);
+                }
 #pragma unroll
                 for (int m = 0; m < M; ++m) {
                     const uint4 xv = reinterpret_cast<const uint4*>(xs + (size_t)m * K)[v];
@@ -122,11 +134,16 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const bf16* __restri
                     }
 #pragma unroll
                     for (int r = 0; r < ROWS; ++r) {
-                        const uint32_t* w32 = reinterpret_cast<const uint32_t*>(&wv[r]);
+                        if constexpr (FP8) {
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            acc[r][m] = fmaf(bf16_lo(w32[j]), xf[2 * j], acc[r][m]);
-                            acc[r][m] = fmaf(bf16_hi(w32[j]), xf[2 * j + 1], acc[r][m]);
+                            for (int j = 0; j < 8; ++j) acc[r][m] = fmaf(wf[r][j], xf[j], acc[r][m]);
+                        } else {
+                            const uint32_t* w32 = reinterpret_cast<const uint32_t*>(&wv[r]);
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {
+                                acc[r][m] = fmaf(bf16_lo(w32[j]), xf[2 * j], acc[r][m]);
+                                acc[r][m] = fmaf(bf16_hi(w32[j]), xf[2 * j + 1], acc[r][m]);
+                            }
                         }
                     }
                 }
@@ -176,10 +193,30 @@ __global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const bf16* __restri
 }
 
 template <int M, int G, int WPI>
-static int launch_gemv(const void* x, const void* W, void* y, int N, int K, const void* bias, const void* residual,
-                       const void* norm_w, float eps, int flags, cudaStream_t st) {
+__global__ void __launch_bounds__(GEMV_THREADS) gemv_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W,
+                                                            bf16* __restrict__ y, int N, int K,
+                                                            const bf16* __restrict__ bias,
+                                                            const bf16* __restrict__ residual,
+                                                            const bf16* __restrict__ norm_w, float eps, int flags) {
+    gemv_body<bf16, M, G, WPI>(x, W, y, N, K, bias, residual, norm_w, eps, flags, nullptr);
+}
+
+template <int M, int G, int WPI>
+__global__ void __launch_bounds__(GEMV_THREADS) gemv_fp8_kernel(const bf16* __restrict__ x,
+                                                                const fp8_e4m3* __restrict__ W, bf16* __restrict__ y,
+                                                                int N, int K, const bf16* __restrict__ bias,
+                                                                const bf16* __restrict__ residual,
+                                                                const bf16* __restrict__ norm_w, float eps, int flags,
+                                                                const float* __restrict__ scales) {
+    gemv_body<fp8_e4m3, M, G, WPI>(x, W, y, N, K, bias, residual, norm_w, eps, flags, scales);
+}
+
+template <typename WT, int M, int G, int WPI>
+static int launch_gemv(const void* x, const void* W, const float* scales, void* y, int N, int K, const void* bias,
+                       const void* residual, const void* norm_w, float eps, int flags, cudaStream_t st) {
     constexpr int SLOTS = GEMV_WARPS / WPI;
-    auto kern = gemv_kernel<M, G, WPI>;
+    constexpr bool FP8 = sizeof(WT) == 1;
+    const void* kern = FP8 ? (const void*)gemv_fp8_kernel<M, G, WPI> : (const void*)gemv_kernel<M, G, WPI>;
     const size_t smem = (size_t)M * K * sizeof(bf16) + (size_t)GEMV_WARPS * 2 * G * M * sizeof(float);
     static bool attr_done = false;   // per instantiation
     if (!attr_done) {
@@ -193,29 +230,35 @@ static int launch_gemv(const void* x, const void* W, void* y, int N, int K, cons
     int grid = (n_items + SLOTS - 1) / SLOTS;
     const int cap = sm_count() * per_sm;
     if (grid > cap) grid = cap;
-    kern<<<grid, GEMV_THREADS, smem, st>>>((const bf16*)x, (const bf16*)W, (bf16*)y, N, K, (const bf16*)bias,
-                                           (const bf16*)residual, (const bf16*)norm_w, eps, flags);
-    return check_launch("tl_gemv_bf16");
+    if constexpr (FP8)
+        gemv_fp8_kernel<M, G, WPI><<<grid, GEMV_THREADS, smem, st>>>((const bf16*)x, (const fp8_e4m3*)W, (bf16*)y, N, K,
+                                                                     (const bf16*)bias, (const bf16*)residual,
+                                                                     (const bf16*)norm_w, eps, flags, scales);
+    else
+        gemv_kernel<M, G, WPI><<<grid, GEMV_THREADS, smem, st>>>((const bf16*)x, (const bf16*)W, (bf16*)y, N, K,
+                                                                 (const bf16*)bias, (const bf16*)residual,
+                                                                 (const bf16*)norm_w, eps, flags);
+    return check_launch(FP8 ? "tl_gemv_fp8" : "tl_gemv_bf16");
 }
 
-template <int M, int G>
-static int dispatch_wpi(int wpi, const void* x, const void* W, void* y, int N, int K, const void* bias,
+template <typename WT, int M, int G>
+static int dispatch_wpi(int wpi, const void* x, const void* W, const float* sc, void* y, int N, int K, const void* bias,
                         const void* residual, const void* norm_w, float eps, int flags, cudaStream_t st) {
     switch (wpi) {
-        case 1: return launch_gemv<M, G, 1>(x, W, y, N, K, bias, residual, norm_w, eps, flags, st);
-        case 2: return launch_gemv<M, G, 2>(x, W, y, N, K, bias, residual, norm_w, eps, flags, st);
-        case 4: return launch_gemv<M, G, 4>(x, W, y, N, K, bias, residual, norm_w, eps, flags, st);
-        default: return launch_gemv<M, G, 8>(x, W, y, N, K, bias, residual, norm_w, eps, flags, st);
+        case 1: return launch_gemv<WT, M, G, 1>(x, W, sc, y, N, K, bias, residual, norm_w, eps, flags, st);
+        case 2: return launch_gemv<WT, M, G, 2>(x, W, sc, y, N, K, bias, residual, norm_w, eps, flags, st);
+        case 4: return launch_gemv<WT, M, G, 4>(x, W, sc, y, N, K, bias, residual, norm_w, eps, flags, st);
+        default: return launch_gemv<WT, M, G, 8>(x, W, sc, y, N, K, bias, residual, norm_w, eps, flags, st);
     }
 }
 
-template <int M>
-static int dispatch_g(int g, int wpi, const void* x, const void* W, void* y, int N, int K, const void* bias,
-                      const void* residual, const void* norm_w, float eps, int flags, cudaStream_t st) {
+template <typename WT, int M>
+static int dispatch_g(int g, int wpi, const void* x, const void* W, const float* sc, void* y, int N, int K,
+                      const void* bias, const void* residual, const void* norm_w, float eps, int flags, cudaStream_t st) {
     switch (g) {
-        case 4: return dispatch_wpi<M, 4>(wpi, x, W, y, N, K, bias, residual, norm_w, eps, flags, st);
-        case 2: return dispatch_wpi<M, 2>(wpi, x, W, y, N, K, bias, residual, norm_w, eps, flags, st);
-        default: return dispatch_wpi<M, 1>(wpi, x, W, y, N, K, bias, residual, norm_w, eps, flags, st);
+        case 4: return dispatch_wpi<WT, M, 4>(wpi, x, W, sc, y, N, K, bias, residual, norm_w, eps, flags, st);
+        case 2: return dispatch_wpi<WT, M, 2>(wpi, x, W, sc, y, N, K, bias, residual, norm_w, eps, flags, st);
+        default: return dispatch_wpi<WT, M, 1>(wpi, x, W, sc, y, N, K, bias, residual, norm_w, eps, flags, st);
     }
 }
 
@@ -224,6 +267,9 @@ int gemv_stream_dispatch(const void* x, const void* W, void* y, int M, int N, in
                          size_t pf_bytes, cudaStream_t st);
 int gemv_mma_dispatch(const void* x, const void* W, void* y, int M, int N, int K, const void* bias, const void* residual,
                       const void* norm_w, float eps, int flags, cudaStream_t st);
+int gemv_stream_fp8_dispatch(const void* x, const void* W, const float* scales, void* y, int M, int N, int K,
+                             const void* bias, const void* residual, const void* norm_w, float eps, int flags, unsigned* ctr,
+                             const void* pf_ptr, size_t pf_bytes, cudaStream_t st);
 
 static bool use_stream_kernel() {
     static int v = -1;
@@ -270,6 +316,55 @@ static unsigned* pool_counter() {
     return g_ctr_pool[dev] + (size_t)i * TL_GEMV_COUNTER_WORDS;
 }
 
+// The passes of one decode Linear call (at most 4 rows each): the weight-streaming kernel, or the register-streaming
+// kernel where x leaves its ring too few stages.  bf16 and FP8 weights take the same kernels, G and WPI on one shape.
+template <typename WT>
+static int gemv_passes(const void* x, const void* W, const float* scales, void* y, int M, int N, int K, const void* bias,
+                       const void* residual, const void* norm_w, float eps, int flags, unsigned* counter,
+                       const void* next_W, size_t next_bytes, cudaStream_t st) {
+    const int nvec = K >> 3;
+    int wpi = 1;
+    while (wpi < 8 && (nvec + 32 * wpi - 1) / (32 * wpi) > 4) wpi <<= 1;
+    const int slots = GEMV_WARPS / wpi;
+    const int npairs = N >> 1;
+    // larger G = more loads in flight per lane; shrink it until there are >= 4 rounds of items per CTA wave
+    int g = 4;
+    const int wave = sm_count() * 2 * slots;
+    while (g > 1 && (npairs / g) < 4 * wave) g >>= 1;
+    const int iters = (nvec + 32 * wpi - 1) / (32 * wpi);
+    if (iters <= 4 && g < 2 && npairs >= 2 * wave) g = 2;
+    // the M template is rounded up to 1/2/4/8 and the surplus rows are never written because the epilogue
+    // indexes only m < M... (rows beyond M would read x out of bounds), so dispatch exactly for 1..4 and
+    // split larger M into two calls.
+    // the launches of one call may overlap under programmatic dependent launch: each takes its own two counter words
+    auto run = [&](int m, const bf16* xx, bf16* yy, const bf16* rr, unsigned* ctr, bool last) -> int {
+        if (use_stream_kernel()) {
+            const void* pf = last ? next_W : nullptr;
+            const size_t pfb = last && next_W ? next_bytes : 0;
+            const int rc = sizeof(WT) == 1
+                ? gemv_stream_fp8_dispatch(xx, W, scales, yy, m, N, K, bias, rr, norm_w, eps, flags, ctr, pf, pfb, st)
+                : gemv_stream_dispatch(xx, W, yy, m, N, K, bias, rr, norm_w, eps, flags, ctr, pf, pfb, st);
+            if (rc != 1) return rc;
+        }
+        switch (m) {
+            case 1: return dispatch_g<WT, 1>(g, wpi, xx, W, scales, yy, N, K, bias, rr, norm_w, eps, flags, st);
+            case 2: return dispatch_g<WT, 2>(g, wpi, xx, W, scales, yy, N, K, bias, rr, norm_w, eps, flags, st);
+            case 3: return dispatch_g<WT, 3>(g, wpi, xx, W, scales, yy, N, K, bias, rr, norm_w, eps, flags, st);
+            default: return dispatch_g<WT, 4>(g, wpi, xx, W, scales, yy, N, K, bias, rr, norm_w, eps, flags, st);
+        }
+    };
+    const int n_out = (flags & TL_EPI_SWIGLU) ? N / 2 : N;
+    int done = 0;
+    while (done < M) {
+        const int m = (M - done) > 4 ? 4 : (M - done);
+        int rc = run(m, (const bf16*)x + (size_t)done * K, (bf16*)y + (size_t)done * n_out,
+                     residual ? (const bf16*)residual + (size_t)done * N : nullptr, counter + 2 * (done / 4), done + m == M);
+        if (rc != TL_OK) return rc;
+        done += m;
+    }
+    return TL_OK;
+}
+
 }  // namespace tl
 
 extern "C" int tl_gemv_bf16_pf(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
@@ -313,42 +408,38 @@ extern "C" int tl_gemv_bf16_ctr(const void* x, const void* W, void* y, int M, in
             if (rc != 1) return rc;
         }
     }
-    const int nvec = K >> 3;
-    int wpi = 1;
-    while (wpi < 8 && (nvec + 32 * wpi - 1) / (32 * wpi) > 4) wpi <<= 1;
-    const int slots = GEMV_WARPS / wpi;
-    const int npairs = N >> 1;
-    // larger G = more loads in flight per lane; shrink it until there are >= 4 rounds of items per CTA wave
-    int g = 4;
-    const int wave = sm_count() * 2 * slots;
-    while (g > 1 && (npairs / g) < 4 * wave) g >>= 1;
-    const int iters = (nvec + 32 * wpi - 1) / (32 * wpi);
-    if (iters <= 4 && g < 2 && npairs >= 2 * wave) g = 2;
-    // the M template is rounded up to 1/2/4/8 and the surplus rows are never written because the epilogue
-    // indexes only m < M... (rows beyond M would read x out of bounds), so dispatch exactly for 1..4 and
-    // split larger M into two calls.
-    // the launches of one call may overlap under programmatic dependent launch: each takes its own two counter words
-    auto run = [&](int m, const bf16* xx, bf16* yy, const bf16* rr, unsigned* ctr, bool last) -> int {
-        if (use_stream_kernel()) {
-            const int rc = gemv_stream_dispatch(xx, W, yy, m, N, K, bias, rr, norm_w, eps, flags, ctr, last ? next_W : nullptr,
-                                                last && next_W ? next_bytes : 0, st);
-            if (rc != 1) return rc;
-        }
-        switch (m) {
-            case 1: return dispatch_g<1>(g, wpi, xx, W, yy, N, K, bias, rr, norm_w, eps, flags, st);
-            case 2: return dispatch_g<2>(g, wpi, xx, W, yy, N, K, bias, rr, norm_w, eps, flags, st);
-            case 3: return dispatch_g<3>(g, wpi, xx, W, yy, N, K, bias, rr, norm_w, eps, flags, st);
-            default: return dispatch_g<4>(g, wpi, xx, W, yy, N, K, bias, rr, norm_w, eps, flags, st);
-        }
-    };
-    const int n_out = (flags & TL_EPI_SWIGLU) ? N / 2 : N;
-    int done = 0;
-    while (done < M) {
-        const int m = (M - done) > 4 ? 4 : (M - done);
-        int rc = run(m, (const bf16*)x + (size_t)done * K, (bf16*)y + (size_t)done * n_out,
-                     residual ? (const bf16*)residual + (size_t)done * N : nullptr, counter + 2 * (done / 4), done + m == M);
-        if (rc != TL_OK) return rc;
-        done += m;
+    return tl::gemv_passes<bf16>(x, W, nullptr, y, M, N, K, bias, residual, norm_w, eps, flags, counter, next_W,
+                                 next_bytes, st);
+}
+
+extern "C" int tl_gemv_fp8(const void* x, const void* W, const float* scales, void* y, int M, int N, int K, const void* bias,
+                           const void* residual, const void* norm_w, float eps, int flags, void* stream) {
+    return tl_gemv_fp8_ctr(x, W, scales, y, M, N, K, bias, residual, norm_w, eps, flags, nullptr, nullptr, 0, stream);
+}
+
+extern "C" int tl_gemv_fp8_ctr(const void* x, const void* W, const float* scales, void* y, int M, int N, int K,
+                               const void* bias, const void* residual, const void* norm_w, float eps, int flags,
+                               unsigned* counter, const void* next_W, size_t next_bytes, void* stream) {
+    using namespace tl;
+    TL_REQUIRE(M >= 1 && M <= 8, TL_ERR_INVALID, "tl_gemv_fp8: M=%d outside 1..8 (dequantize and use tl_gemm_bf16)", M);
+    TL_REQUIRE(((uintptr_t)counter & 3) == 0, TL_ERR_INVALID, "tl_gemv_fp8: counter block not 4-byte aligned");
+    TL_REQUIRE(K % TL_FP8_BLOCK == 0 && N % 2 == 0 && N > 0 && K > 0, TL_ERR_INVALID,
+               "tl_gemv_fp8: need K %% %d == 0 and N even (N=%d K=%d)", TL_FP8_BLOCK, N, K);
+    TL_REQUIRE(((uintptr_t)W & 15) == 0 && ((uintptr_t)scales & 3) == 0 && scales, TL_ERR_INVALID,
+               "tl_gemv_fp8: W must be 16-byte aligned and scales non-NULL and 4-byte aligned");
+    TL_REQUIRE(!(flags & ~(TL_EPI_BIAS | TL_EPI_RESIDUAL | TL_EPI_SWIGLU)), TL_ERR_INVALID,
+               "tl_gemv_fp8: unsupported flags 0x%x", flags);
+    TL_REQUIRE(!((flags & TL_EPI_SWIGLU) && (flags & TL_EPI_RESIDUAL)), TL_ERR_INVALID,
+               "tl_gemv_fp8: SWIGLU and RESIDUAL are exclusive");
+    TL_REQUIRE(!(flags & TL_EPI_BIAS) || bias, TL_ERR_INVALID, "tl_gemv_fp8: BIAS flag without bias pointer");
+    TL_REQUIRE(!(flags & TL_EPI_RESIDUAL) || residual, TL_ERR_INVALID, "tl_gemv_fp8: RESIDUAL flag without pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!counter) {
+        counter = pool_counter();
+        if (!counter) cudaGetLastError();
+        TL_REQUIRE(counter, TL_ERR_CUDA, "tl_gemv_fp8: allocating the counter pool failed (first call on this device "
+                   "inside a graph capture?)");
     }
-    return TL_OK;
+    return gemv_passes<fp8_e4m3>(x, W, scales, y, M, N, K, bias, residual, norm_w, eps, flags, counter, next_W,
+                                 next_bytes, st);
 }

@@ -11,9 +11,16 @@
 // cross-warp traffic.  x (optionally RMS-normalised with HF rounding) is staged once per CTA while the producer is
 // already streaming.
 // Algorithmic bytes per launch = 2*N*K.
+//
+// The same kernel streams FP8 weights (WT = fp8_e4m3, tl_gemv_fp8): one byte per weight plus an fp32 scale per (row,
+// 128-column group), read through L1.  Each weight is formed as bf16(float(w) * scale), the bf16 weight of HF's
+// dequantized checkpoint, and every lane visits K in the bf16 kernel's order (lane v of a pass takes elements 8v..8v+7),
+// so the FMA sequence of every output, and therefore the result, is the bf16 kernel's over the dequantized matrix.
+// A stage then holds twice the rows, and a chunk of a chunked pair twice the columns.
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "fp8.cuh"
 
 namespace tl {
 
@@ -21,7 +28,8 @@ constexpr int GS_CONSUMER_WARPS = 8;
 constexpr int GS_THREADS = (GS_CONSUMER_WARPS + 1) * 32;
 constexpr int GS_MAX_STAGES = 16;
 constexpr int GS_STAGE_BYTES = 16 * 1024;
-constexpr int GS_KC = 4096;            // K chunk (elements) when a pair does not fit one stage
+constexpr int GS_KC = 4096;            // K chunk (elements of a bf16 weight) when a pair does not fit one stage
+constexpr int GS_SCALE_GROUP = 128;    // FP8 weights: one fp32 scale per row and 128 consecutive columns
 // Bytes per ticket: one atomic round trip (~1 us under a full HBM stream) has to hide behind the ticket before it, and
 // a CTA finishes at most one ticket after the others.
 constexpr int GS_TICKET_BYTES = 24 * 1024;
@@ -32,12 +40,16 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-template <int M>
-__global__ void __launch_bounds__(GS_THREADS, 1)
-gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16* __restrict__ y, int N, int K,
-                   const bf16* __restrict__ bias, const bf16* __restrict__ residual, const bf16* __restrict__ norm_w,
-                   float eps, int flags, int P, int n_stages, int NW, int stage_bytes, int G, unsigned* __restrict__ ctr,
-                   const unsigned char* __restrict__ pf_ptr, unsigned long long pf_bytes) {
+// The body of both kernels below.  WT: bf16, or fp8_e4m3 with `scales` [N][K/128].
+template <typename WT, int M>
+__device__ __forceinline__ void
+gemv_stream_body(const bf16* __restrict__ x, const WT* __restrict__ W, bf16* __restrict__ y, int N, int K,
+                 const bf16* __restrict__ bias, const bf16* __restrict__ residual, const bf16* __restrict__ norm_w,
+                 float eps, int flags, int P, int n_stages, int NW, int stage_bytes, int G, unsigned* __restrict__ ctr,
+                 const unsigned char* __restrict__ pf_ptr, unsigned long long pf_bytes, const float* __restrict__ scales) {
+    constexpr bool FP8 = sizeof(WT) == 1;
+    constexpr int WB = sizeof(WT);                 // bytes per weight
+    constexpr int KCW = GS_KC * 2 / WB;            // chunk columns: a chunk of a pair fills one 16 KB stage
     extern __shared__ __align__(128) unsigned char smem[];
     unsigned char* ring = smem;                                                    // [n_stages][stage_bytes]
     bf16* xs = reinterpret_cast<bf16*>(smem + (size_t)n_stages * stage_bytes);     // [M][K]
@@ -53,8 +65,8 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
     const int n_units = (npairs + P - 1) / P;                          // unit = P consecutive pairs
     // NW consumer warps take units; n_stages %% NW == 0, so ring slot s is ALWAYS consumed by warp s %% NW and every
     // waiter observes every phase of the barriers it waits on (no mbarrier parity aliasing).
-    const bool chunked = K > GS_KC || (size_t)K * 4 > GS_STAGE_BYTES;  // a pair does not fit one stage
-    const int KC = chunked ? GS_KC : K;
+    const bool chunked = K > KCW || (size_t)K * (2 * WB) > GS_STAGE_BYTES;  // a pair does not fit one stage
+    const int KC = chunked ? KCW : K;
     const int n_chunks = (K + KC - 1) / KC;
 
     if (tid == 0) {
@@ -119,15 +131,15 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
                             } else if (!chunked) {   // np pairs = 2*np whole rows, contiguous in memory: one copy
                                 const int pair0 = unit[w] * P;
                                 const int np = min(P, npairs - pair0);
-                                const uint32_t bytes = (uint32_t)(2 * np) * (uint32_t)K * 2u;
+                                const uint32_t bytes = (uint32_t)(2 * np) * (uint32_t)K * (uint32_t)WB;
                                 mbar_expect_tx(&full_bar[stage], bytes);
                                 bulk_load_1d(dst, W + (size_t)(2 * pair0) * K, bytes, &full_bar[stage]);
                             } else {                 // one K chunk of the two rows of one pair: two copies
                                 const int k0 = chunk[w] * KC;
-                                const uint32_t bytes = (uint32_t)min(KC, K - k0) * 2u;
+                                const uint32_t bytes = (uint32_t)min(KC, K - k0) * (uint32_t)WB;
                                 mbar_expect_tx(&full_bar[stage], 2 * bytes);
                                 bulk_load_1d(dst, W + (size_t)(2 * unit[w]) * K + k0, bytes, &full_bar[stage]);
-                                bulk_load_1d(dst + (size_t)KC * 2, W + (size_t)(2 * unit[w] + 1) * K + k0, bytes, &full_bar[stage]);
+                                bulk_load_1d(dst + (size_t)KC * WB, W + (size_t)(2 * unit[w] + 1) * K + k0, bytes, &full_bar[stage]);
                                 if (++chunk[w] == n_chunks) chunk[w] = 0;
                             }
                         }
@@ -237,11 +249,36 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
                 }
             }
         };
-        // dot product of `vecs` 16-byte vectors of two rows against x[k0..]
-        auto dot2 = [&](const uint4* r0, const uint4* r1, int k0, int vecs, float (&a0)[M], float (&a1)[M]) {
+        // dot product of `vecs` 8-weight vectors of two rows (stage rows r0, r1 = W rows row0, row0 + 1) against x[k0..]
+        auto dot2 = [&](const unsigned char* r0, const unsigned char* r1, int row0, int k0, int vecs, float (&a0)[M],
+                        float (&a1)[M]) {
+          if constexpr (FP8) {
+            const int n_groups = K / GS_SCALE_GROUP;
+            const float* s0 = scales + (size_t)row0 * n_groups + k0 / GS_SCALE_GROUP;
+            const float* s1 = s0 + n_groups;
 #pragma unroll 4
             for (int v = lane; v < vecs; v += 32) {
-                const uint4 w0 = r0[v], w1 = r1[v];
+                float w0[8], w1[8];
+                fp8x8_scaled(reinterpret_cast<const uint2*>(r0)[v], __ldg(s0 + (v >> 4)), w0);
+                fp8x8_scaled(reinterpret_cast<const uint2*>(r1)[v], __ldg(s1 + (v >> 4)), w1);
+#pragma unroll
+                for (int m = 0; m < M; ++m) {
+                    const uint4 xv = reinterpret_cast<const uint4*>(xs + (size_t)m * K + k0)[v];
+                    const uint32_t* x32 = reinterpret_cast<const uint32_t*>(&xv);
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const float xl = bf16_lo(x32[j]), xh = bf16_hi(x32[j]);
+                        a0[m] = fmaf(w0[2 * j], xl, a0[m]);
+                        a0[m] = fmaf(w0[2 * j + 1], xh, a0[m]);
+                        a1[m] = fmaf(w1[2 * j], xl, a1[m]);
+                        a1[m] = fmaf(w1[2 * j + 1], xh, a1[m]);
+                    }
+                }
+            }
+          } else {
+#pragma unroll 4
+            for (int v = lane; v < vecs; v += 32) {
+                const uint4 w0 = reinterpret_cast<const uint4*>(r0)[v], w1 = reinterpret_cast<const uint4*>(r1)[v];
                 const uint32_t* a32 = reinterpret_cast<const uint32_t*>(&w0);
                 const uint32_t* b32 = reinterpret_cast<const uint32_t*>(&w1);
 #pragma unroll
@@ -258,6 +295,7 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
                     }
                 }
             }
+          }
         };
         // this warp's stages are sequence numbers warp, warp+NW, warp+2*NW, ... of the producer's order; the producer
         // says in s_unit which unit each one holds
@@ -279,16 +317,15 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
                     float b0[M], b1[M];
 #pragma unroll
                     for (int m = 0; m < M; ++m) b0[m] = b1[m] = 0.f;
-                    dot2(reinterpret_cast<const uint4*>(src + (size_t)(2 * pp) * K * 2),
-                         reinterpret_cast<const uint4*>(src + (size_t)(2 * pp + 1) * K * 2), 0, nvec, b0, b1);
+                    dot2(src + (size_t)(2 * pp) * K * WB, src + (size_t)(2 * pp + 1) * K * WB, 2 * (pair0 + pp), 0, nvec,
+                         b0, b1);
 #pragma unroll
                     for (int m = 0; m < M; ++m) { b0[m] = warp_sum(b0[m]); b1[m] = warp_sum(b1[m]); }
                     finish(pair0 + pp, b0, b1);
                 }
             } else if (unit >= 0) {
                 const int k0 = c * KC;
-                dot2(reinterpret_cast<const uint4*>(src), reinterpret_cast<const uint4*>(src + (size_t)KC * 2), k0,
-                     min(KC, K - k0) >> 3, a0, a1);
+                dot2(src, src + (size_t)KC * WB, 2 * unit, k0, min(KC, K - k0) >> 3, a0, a1);
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&empty_bar[stage]);
@@ -306,10 +343,34 @@ gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16*
 }
 
 template <int M>
-static int launch_stream(const void* x, const void* W, void* y, int N, int K, const void* bias, const void* residual,
-                         const void* norm_w, float eps, int flags, unsigned* ctr, const void* pf_ptr, size_t pf_bytes,
-                         cudaStream_t st) {
-    auto kern = gemv_stream_kernel<M>;
+__global__ void __launch_bounds__(GS_THREADS, 1)
+gemv_stream_kernel(const bf16* __restrict__ x, const bf16* __restrict__ W, bf16* __restrict__ y, int N, int K,
+                   const bf16* __restrict__ bias, const bf16* __restrict__ residual, const bf16* __restrict__ norm_w,
+                   float eps, int flags, int P, int n_stages, int NW, int stage_bytes, int G, unsigned* __restrict__ ctr,
+                   const unsigned char* __restrict__ pf_ptr, unsigned long long pf_bytes) {
+    gemv_stream_body<bf16, M>(x, W, y, N, K, bias, residual, norm_w, eps, flags, P, n_stages, NW, stage_bytes, G, ctr,
+                              pf_ptr, pf_bytes, nullptr);
+}
+
+template <int M>
+__global__ void __launch_bounds__(GS_THREADS, 1)
+gemv_stream_fp8_kernel(const bf16* __restrict__ x, const fp8_e4m3* __restrict__ W, bf16* __restrict__ y, int N, int K,
+                       const bf16* __restrict__ bias, const bf16* __restrict__ residual, const bf16* __restrict__ norm_w,
+                       float eps, int flags, int P, int n_stages, int NW, int stage_bytes, int G,
+                       unsigned* __restrict__ ctr, const unsigned char* __restrict__ pf_ptr, unsigned long long pf_bytes,
+                       const float* __restrict__ scales) {
+    gemv_stream_body<fp8_e4m3, M>(x, W, y, N, K, bias, residual, norm_w, eps, flags, P, n_stages, NW, stage_bytes, G,
+                                  ctr, pf_ptr, pf_bytes, scales);
+}
+
+template <typename WT, int M>
+static int launch_stream(const void* x, const void* W, const float* scales, void* y, int N, int K, const void* bias,
+                         const void* residual, const void* norm_w, float eps, int flags, unsigned* ctr, const void* pf_ptr,
+                         size_t pf_bytes, cudaStream_t st) {
+    constexpr size_t WB = sizeof(WT);
+    const char* what = WB == 1 ? "tl_gemv_fp8/stream" : "tl_gemv_bf16/stream";
+    constexpr bool FP8 = WB == 1;
+    void* kern = FP8 ? (void*)gemv_stream_fp8_kernel<M> : (void*)gemv_stream_kernel<M>;
     // Two half-size rings per SM (16 consumer warps, finer work split, the next kernel's CTAs become resident as soon as
     // one of the two exits) when an SM's share of W is small — the latency-bound regime of small models; one deep
     // ring per SM otherwise.  The 128 KB threshold has not been re-chosen by measurement on H100.
@@ -319,7 +380,7 @@ static int launch_stream(const void* x, const void* W, void* y, int N, int K, co
         const char* e = getenv("TL_GEMV_CTAS_PER_SM");
         forced = (e && e[0] == '2') ? 2 : ((e && e[0] == '1') ? 1 : 0);
     }
-    const int per_sm = forced ? forced : (((size_t)N * K * 2 / (size_t)sm_count() <= (size_t)128 * 1024) ? 2 : 1);
+    int per_sm = forced ? forced : (((size_t)N * K * WB / (size_t)sm_count() <= (size_t)128 * 1024) ? 2 : 1);
     // TL_GEMV_RING_KB (default 220): shared memory per CTA.  <= 110 leaves room for the NEXT kernel's CTA on the same
     // SM, so under programmatic dependent launch its producer fills its ring while this kernel is still streaming.
     static int ring_kb = 0;
@@ -328,21 +389,37 @@ static int launch_stream(const void* x, const void* W, void* y, int N, int K, co
         ring_kb = e ? atoi(e) : 220;
         if (ring_kb < 48 || ring_kb > 220) ring_kb = 220;
     }
+    const size_t xs_bytes = (((size_t)M * K * 2) + 15) & ~(size_t)15;
+    const size_t fixed = xs_bytes + 2 * GS_MAX_STAGES * sizeof(uint64_t);
+    if constexpr (FP8) {
+        // The FP8 kernel runs exactly where the bf16 kernel would run on this shape, and the register-streaming
+        // fallback everywhere else, so an FP8 GEMV takes the kernel (and the summation order) of the bf16 GEMV over the
+        // dequantized weights.  Its own ring then takes one CTA per SM when two half-size rings would be too shallow.
+        auto stages = [&](int wb, int ps) -> int64_t {
+            const bool ch = K > GS_KC * 2 / wb || (size_t)K * 2 * wb > GS_STAGE_BYTES;
+            int p = ch ? 1 : (int)(GS_STAGE_BYTES / ((size_t)K * 2 * wb));
+            p = p < 1 ? 1 : (p > 8 ? 8 : p);
+            const int64_t sb = ch ? GS_STAGE_BYTES : (int64_t)((((size_t)p * K * 2 * wb) + 127) & ~(size_t)127);
+            return ((int64_t)(ps == 2 ? 110 * 1024 : ring_kb * 1024) - (int64_t)fixed) / sb;
+        };
+        const int per_sm_bf16 = forced ? forced : (((size_t)N * K * 2 / (size_t)sm_count() <= (size_t)128 * 1024) ? 2 : 1);
+        if (stages(2, per_sm_bf16) < 4) return 1;
+        if (per_sm == 2 && stages(1, 2) < 4) per_sm = 1;
+    }
     const int SMEM_CAP = per_sm == 2 ? 110 * 1024 : ring_kb * 1024;
     static bool attr_done = false;
     if (!attr_done) {
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024) != cudaSuccess)
-            return check_launch("tl_gemv_bf16/stream (smem attr)");
+        if (cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024) != cudaSuccess)
+            return check_launch(what);
         attr_done = true;
     }
-    const size_t xs_bytes = (((size_t)M * K * 2) + 15) & ~(size_t)15;
-    const size_t fixed = xs_bytes + 2 * GS_MAX_STAGES * sizeof(uint64_t);
-    const bool chunked = K > GS_KC || (size_t)K * 4 > GS_STAGE_BYTES;
-    int P = chunked ? 1 : (int)(GS_STAGE_BYTES / ((size_t)K * 4));
+    const int KCW = GS_KC * 2 / (int)WB;
+    const bool chunked = K > KCW || (size_t)K * 2 * WB > GS_STAGE_BYTES;
+    int P = chunked ? 1 : (int)(GS_STAGE_BYTES / ((size_t)K * 2 * WB));
     if (P < 1) P = 1;
     if (P > 8) P = 8;
-    // a stage holds one unit: up to P whole pairs, or one 4096-column chunk of one pair
-    const int stage_bytes = chunked ? GS_STAGE_BYTES : (int)((((size_t)P * K * 4) + 127) & ~(size_t)127);
+    // a stage holds one unit: up to P whole pairs, or one 16 KB chunk of one pair
+    const int stage_bytes = chunked ? GS_STAGE_BYTES : (int)((((size_t)P * K * 2 * WB) + 127) & ~(size_t)127);
     int max_stages = (int)((SMEM_CAP - fixed) / stage_bytes);
     if (max_stages > GS_MAX_STAGES) max_stages = GS_MAX_STAGES;
     if (max_stages < 4) return 1;   // caller falls back to the register-streaming kernel
@@ -363,7 +440,7 @@ static int launch_stream(const void* x, const void* W, void* y, int N, int K, co
         P = 1;
         G = (npairs + grid - 1) / grid;
     } else {
-        const int unit_bytes = chunked ? K * 4 : P * K * 4;
+        const int unit_bytes = (int)(chunked ? K * 2 * WB : P * K * 2 * WB);
         G = (GS_TICKET_BYTES + unit_bytes - 1) / unit_bytes;
     }
     cudaLaunchConfig_t cfg = {};
@@ -381,25 +458,46 @@ static int launch_stream(const void* x, const void* W, void* y, int N, int K, co
     }
     cfg.attrs = attr;
     cfg.numAttrs = use_pdl ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, kern, (const bf16*)x, (const bf16*)W, (bf16*)y, N, K, (const bf16*)bias, (const bf16*)residual,
-                       (const bf16*)norm_w, eps, flags, P, n_stages, NW, stage_bytes, G, ctr, (const unsigned char*)pf_ptr,
-                       (unsigned long long)(pf_bytes & ~(size_t)15));
-    return check_launch("tl_gemv_bf16/stream");
+    if constexpr (FP8)
+        cudaLaunchKernelEx(&cfg, gemv_stream_fp8_kernel<M>, (const bf16*)x, (const fp8_e4m3*)W, (bf16*)y, N, K,
+                           (const bf16*)bias, (const bf16*)residual, (const bf16*)norm_w, eps, flags, P, n_stages, NW,
+                           stage_bytes, G, ctr, (const unsigned char*)pf_ptr, (unsigned long long)(pf_bytes & ~(size_t)15),
+                           scales);
+    else
+        cudaLaunchKernelEx(&cfg, gemv_stream_kernel<M>, (const bf16*)x, (const bf16*)W, (bf16*)y, N, K, (const bf16*)bias,
+                           (const bf16*)residual, (const bf16*)norm_w, eps, flags, P, n_stages, NW, stage_bytes, G, ctr,
+                           (const unsigned char*)pf_ptr, (unsigned long long)(pf_bytes & ~(size_t)15));
+    return check_launch(what);
+}
+
+template <typename WT>
+static int stream_dispatch(const void* x, const void* W, const float* scales, void* y, int M, int N, int K,
+                           const void* bias, const void* residual, const void* norm_w, float eps, int flags, unsigned* ctr,
+                           const void* pf_ptr, size_t pf_bytes, cudaStream_t st) {
+    if (K % 8 != 0 || ((uintptr_t)W & 15)) return 1;
+    if ((uintptr_t)pf_ptr & 15) pf_bytes = 0;
+    switch (M) {
+        case 1: return launch_stream<WT, 1>(x, W, scales, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
+        case 2: return launch_stream<WT, 2>(x, W, scales, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
+        case 3: return launch_stream<WT, 3>(x, W, scales, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
+        case 4: return launch_stream<WT, 4>(x, W, scales, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
+        default: return 1;
+    }
 }
 
 // returns TL_OK, an error, or 1 = "not applicable, use the fallback kernel"
 int gemv_stream_dispatch(const void* x, const void* W, void* y, int M, int N, int K, const void* bias,
                          const void* residual, const void* norm_w, float eps, int flags, unsigned* ctr, const void* pf_ptr,
                          size_t pf_bytes, cudaStream_t st) {
-    if (K % 8 != 0 || ((uintptr_t)W & 15)) return 1;
-    if ((uintptr_t)pf_ptr & 15) pf_bytes = 0;
-    switch (M) {
-        case 1: return launch_stream<1>(x, W, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
-        case 2: return launch_stream<2>(x, W, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
-        case 3: return launch_stream<3>(x, W, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
-        case 4: return launch_stream<4>(x, W, y, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
-        default: return 1;
-    }
+    return stream_dispatch<bf16>(x, W, nullptr, y, M, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes, st);
+}
+
+// FP8 weights (scales [N][K/128] fp32): TL_OK, an error, or 1 = "the shapes do not fit the stream kernel"
+int gemv_stream_fp8_dispatch(const void* x, const void* W, const float* scales, void* y, int M, int N, int K,
+                             const void* bias, const void* residual, const void* norm_w, float eps, int flags, unsigned* ctr,
+                             const void* pf_ptr, size_t pf_bytes, cudaStream_t st) {
+    return stream_dispatch<fp8_e4m3>(x, W, scales, y, M, N, K, bias, residual, norm_w, eps, flags, ctr, pf_ptr, pf_bytes,
+                                     st);
 }
 
 }  // namespace tl

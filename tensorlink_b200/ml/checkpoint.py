@@ -5,7 +5,9 @@ remaps their keys to the local module (/root/reference/tensorlink/ml/worker.py:5
 gathers parameters back through ``parameters(distributed=True)`` (ml/module.py:577-650).  Here a stage asks a
 ``LazyCheckpoint`` for exactly the HF tensor names it owns — nothing else is read from disk — and
 ``save_checkpoint`` writes one ``model-XXXXX-of-YYYYY.safetensors`` per stage plus the index and ``config.json``, so
-the directory loads back here, in the reference, or in ``transformers``.
+the directory loads back here, in the reference, or in ``transformers``.  An FP8 model (ml/fp8.py) reads and writes HF's
+fine-grained FP8 layout: ``...weight`` in float8_e4m3fn, ``...weight_scale_inv`` per 128x128 block and a
+``quantization_config`` in ``config.json``.
 """
 from __future__ import annotations
 
@@ -15,16 +17,26 @@ from typing import Dict, Iterator
 
 import torch
 
+from . import fp8 as F8
 from .configs import ShardModelConfig
 
 INDEX = "model.safetensors.index.json"
 SINGLE = "model.safetensors"
 
 
+def quantization_from_dir(path: str):
+    """The checkpoint's ``quantization_config`` parsed by ``ml/fp8.parse_quantization_config`` (None for a bf16
+    checkpoint); variants this project does not run raise NotImplementedError."""
+    with open(os.path.join(path, "config.json")) as f:
+        return F8.parse_quantization_config(json.load(f).get("quantization_config"))
+
+
 def config_from_dir(path: str) -> ShardModelConfig:
-    """``config.json`` (HF Qwen2 / Qwen3 causal LM) -> ShardModelConfig."""
+    """``config.json`` (HF Qwen2 / Qwen3 causal LM, bf16 or HF's fine-grained FP8) -> ShardModelConfig.  An FP8
+    ``quantization_config`` the project does not run raises NotImplementedError (``quantization_from_dir``)."""
     with open(os.path.join(path, "config.json")) as f:
         c = json.load(f)
+    quantization_from_dir(path)
     mt = c.get("model_type", "")
     if mt not in ("qwen2", "qwen3"):
         raise ValueError(f"{path}: model_type {mt!r} is not supported (qwen2 / qwen3)")
@@ -110,5 +122,8 @@ def save_checkpoint(dm, path: str, link=None) -> None:
         with open(os.path.join(path, INDEX), "w") as f:
             json.dump({"metadata": {"total_size": int(sum(sizes))}, "weight_map": weight_map}, f, indent=1)
         with open(os.path.join(path, "config.json"), "w") as f:
-            json.dump(config_to_json(dm.cfg), f, indent=1)
+            c = config_to_json(dm.cfg)
+            if getattr(dm, "quantization", None):
+                c["quantization_config"] = F8.config_dict()
+            json.dump(c, f, indent=1)
     link.barrier()

@@ -24,6 +24,7 @@ import torch
 
 from ..native import LP_MAX_EOS, PL_MAX_DRAFT, PL_MAX_EOS
 from ..p2p.link import StageLink, init_process_group_from_env
+from . import fp8 as F8
 from . import graphing
 from .configs import ShardModelConfig, get_config
 
@@ -290,23 +291,45 @@ class DistributedModel(torch.nn.Module):
                  training: bool = True, verbose: bool = False, tokenizer=None, config: Optional[dict] = None,
                  *, max_batch: int = 8, max_seq: int = 4096, seed: int = 1234, init: str = "seeded",
                  balanced_plan: bool = False, link: Optional[StageLink] = None, max_tokens: Optional[int] = None,
-                 _stage_factory: Optional[Callable] = None):
+                 quantization_config=None, _stage_factory: Optional[Callable] = None):
+        """``model``: an HF Qwen2 / Qwen3 module, a ShardModelConfig or registered config name (weights drawn by
+        ``init``: "seeded" or "device"), or a local HF checkpoint directory, bf16 or in HF's fine-grained FP8 layout
+        (``quantization_config.quant_method == "fp8"``, e4m3, 128x128 blocks; each stage reads its own ``weight`` and
+        ``weight_scale_inv`` tensors).
+
+        ``quantization_config``: HF's ``FineGrainedFP8Config`` or the same dict.  It quantizes the decoder layers'
+        Linears of an in-memory bf16 model on load with HF's rule (``Fp8Quantize``).  FP8 models run weight-only (W8A16):
+        each weight is bf16(float32(w) * scale_inv[block]), so their outputs equal, bit for bit, those of the bf16 model
+        over HF's dequantized weights (``FineGrainedFP8Config(dequantize=True)``).  HF's GPU ``FP8Linear`` also
+        quantizes the activations per 1x128 group; that is deliberately not done here.  Norms, biases, the embedding
+        and the lm_head stay bf16.  Training FP8 weights is not supported: pass ``training=False``."""
         super().__init__()
         if dtype != torch.bfloat16:
             raise NotImplementedError("tensorlink_b200 computes in bf16 with fp32 accumulation; pass dtype=torch.bfloat16")
+        quantization = F8.parse_quantization_config(quantization_config)
         state_dict = None
         if isinstance(model, torch.nn.Module):
             self.cfg = _config_from_hf(model)
             state_dict = model.state_dict()
+            if any(t.dtype == torch.float8_e4m3fn for t in state_dict.values()):
+                # an HF module loaded with FineGrainedFP8Config: its Linears hold e4m3 codes + weight_scale_inv
+                hf_q = getattr(model.config, "quantization_config", None)
+                if hf_q is None:
+                    raise NotImplementedError("an HF module with float8 weights but no config.quantization_config")
+                quantization = F8.parse_quantization_config(hf_q)
         elif isinstance(model, ShardModelConfig):
             self.cfg = model
         elif isinstance(model, str) and os.path.isdir(model) and os.path.exists(os.path.join(model, "config.json")):
             # a local checkpoint in the HF layout: each stage reads only its own tensors (worker.py:542-638)
-            from .checkpoint import LazyCheckpoint, config_from_dir
+            from .checkpoint import LazyCheckpoint, config_from_dir, quantization_from_dir
             self.cfg = config_from_dir(model)
+            quantization = quantization_from_dir(model) or quantization
             state_dict = LazyCheckpoint(model)
         else:
             self.cfg = get_config(model)
+        if quantization is not None and training:
+            raise NotImplementedError("training with FP8 weights is not supported: load an FP8 model with training=False")
+        self.quantization = quantization
         self.model_name = self.cfg.name
         self.name = self.model_name
         self.tokenizer = tokenizer
@@ -365,7 +388,8 @@ class DistributedModel(torch.nn.Module):
                                          max_batch=per_slot, max_seq=self.max_seq, n_slots=n_slots,
                                          training=self.training, state_dict=self._stage_kw["state_dict"],
                                          seed=self.seed, init=self._stage_kw["init"],
-                                         max_tokens=self._stage_kw["max_tokens"])
+                                         max_tokens=self._stage_kw["max_tokens"],
+                                         **({"quantization": self.quantization} if self.quantization else {}))
         self._stage_kw["state_dict"] = None
         return plan
 
@@ -404,6 +428,8 @@ class DistributedModel(torch.nn.Module):
         save_checkpoint(self, path)
 
     def create_optimizer(self, **optimizer_kwargs):
+        if self.quantization is not None:
+            raise NotImplementedError("training with FP8 weights is not supported (no optimizer for an FP8 model)")
         from .optim import create_distributed_optimizer
         return create_distributed_optimizer(self, self.optimizer, **optimizer_kwargs)
 
@@ -620,6 +646,9 @@ class DistributedModel(torch.nn.Module):
         order and before the sampling warpers, on the last stage's GPU inside the decode graph (csrc/logits_process.cu).
         As in HF the history they look at is the whole ``input_ids`` row, pad tokens included, plus the generated tokens.
         ``input_ids`` [B,S] int64 on the first stage; returns [B,S+new] on every rank.
+        An FP8 model (``quantization_config``, or an FP8 checkpoint) generates through every mode here with the tokens
+        of the bf16 model over HF's dequantized weights: decode and verify steps of few rows stream the FP8 weights
+        (``shard.fp8_gemv_rows``), larger ones dequantize each Linear before the bf16 GEMM.
         ``streamer``: object with ``put(tensor)`` / ``end()`` (HF BaseStreamer protocol), called on rank 0
         with each new token column, all batch rows (the reference streams row 0 only, worker.py:134-139).
         ``attention_mask``: a left-padded batch (HF's layout for batched generation) runs as ONE batch: columns that are

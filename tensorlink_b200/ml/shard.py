@@ -11,6 +11,9 @@ HBM layout (per shard):
   params   one flat bf16 arena; per layer  ln1 | wqkv[(n_h+2n_kv)d, H] | bqkv | (q_norm,k_norm) | wo[H, n_h d] |
            ln2 | wgu[2I, H] (row 2j = gate_j, row 2j+1 = up_j) | wd[H, I]; then embed / final norm / lm_head
            on the ranks that own them.  Every tensor starts on a 256-byte boundary (TMA needs 16).
+  fp8      FP8 shards (``ShardParams(fp8=True)``, ml/fp8.py): the four Linear weights of every layer live instead in a
+           float8_e4m3fn arena in the same row layout (256-byte boundaries), with fp32 scales [N, K/128] per row in a
+           third arena; norms, biases, embed, final norm and lm_head stay in the bf16 arena.
   kv       per layer K and V  [B_max, n_kv, T_max, d] bf16 (head-major: decode streams [T, d] per head).
   act      x[N,H], qkv[N,(n_h+2n_kv)d], q[N,n_h d], attn[N,n_h d], h[N,H], act[N,I]  for N = B*S tokens.
 """
@@ -22,6 +25,7 @@ from typing import Dict, List, Optional, Sequence
 import torch
 
 from .. import native as nat
+from . import fp8 as F8
 from .configs import ShardModelConfig
 from .weights import init_state_dict
 
@@ -42,6 +46,34 @@ def gemv_max_rows() -> int:
     return _GEMV_MAX_ROWS
 
 
+_FP8_GEMV_MAX_ROWS = None
+
+
+def fp8_gemv_max_rows() -> int:
+    """``gemv_max_rows()`` for FP8 shards: rows per step up to which the FP8 weight-streaming GEMV runs (in passes of at
+    most 4 rows, one byte per weight each); more rows dequantize each Linear into a bf16 scratch buffer and run the GEMM
+    path (about 5 bytes per weight).  Default 4, one GEMV pass: measured on an H100 SXM (700 W) with tools/bench_fp8.py,
+    the GEMV wins at 4 rows for Qwen2.5-7B and Qwen3-8B, while at 6..8 rows (two passes) the two models disagree
+    (DESIGN.md §4.1).  TL_FP8_GEMV_MAX_ROWS overrides (1..8)."""
+    global _FP8_GEMV_MAX_ROWS
+    if _FP8_GEMV_MAX_ROWS is None:
+        import os
+        _FP8_GEMV_MAX_ROWS = max(1, min(8, int(os.environ.get("TL_FP8_GEMV_MAX_ROWS", "4"))))
+    return _FP8_GEMV_MAX_ROWS
+
+
+def fp8_gemv_rows(cfg: ShardModelConfig) -> int:
+    """Rows per step up to which an FP8 stage of ``cfg`` runs the FP8 GEMV: ``fp8_gemv_max_rows()``, lowered so that
+    one pass (at most 4 rows) of staged activations fits the register-streaming kernel's shared memory for the widest
+    Linear input (the down projection's K = intermediate).  That kernel is where a pass goes when x leaves the
+    weight-streaming ring too few stages, as for the bf16 GEMV; past it the step takes the dequantize + GEMM path."""
+    K = max(cfg.hidden, cfg.q_dim, cfg.intermediate)
+    fit = 0
+    while fit < 4 and (fit + 1) * K * 2 + 256 * (fit + 1) <= 200 * 1024:       # x rows + the epilogue's partial sums
+        fit += 1
+    return min(fp8_gemv_max_rows(), fit)
+
+
 def _rope_inv_freq(cfg: ShardModelConfig) -> torch.Tensor:
     """site-packages/transformers/models/qwen2/modeling_qwen2.py:84-99, computed on the host in fp32 like HF."""
     d = cfg.head_dim
@@ -49,10 +81,14 @@ def _rope_inv_freq(cfg: ShardModelConfig) -> torch.Tensor:
 
 
 class ShardParams:
-    """Flat bf16 parameter arena of one shard, with fused-QKV / interleaved gate-up views."""
+    """Flat bf16 parameter arena of one shard, with fused-QKV / interleaved gate-up views.  ``fp8=True``: the decoder
+    layers' Linear weights are float8_e4m3fn views (``v``) with per-row scales (``s``), see the module docstring."""
 
     def __init__(self, cfg: ShardModelConfig, layer_ids: Sequence[int], has_embed: bool, has_head: bool,
-                 device, with_grad: bool = False):
+                 device, with_grad: bool = False, fp8: bool = False):
+        if fp8 and with_grad:
+            raise NotImplementedError("training with FP8 weights is not supported (load the model with training=False)")
+        self.fp8 = bool(fp8)
         self.cfg, self.layer_ids = cfg, list(layer_ids)
         self.has_embed, self.has_head = has_embed, has_head
         self.device = torch.device(device)
@@ -72,6 +108,8 @@ class ShardParams:
             spec.append(("norm", (H,)))
             if not (cfg.tied and has_embed):
                 spec.append(("head", (cfg.vocab, H)))
+        qspec = [(n, sh) for n, sh in spec if n.split(".")[-1] in F8.LINEARS] if self.fp8 else []
+        spec = [(n, sh) for n, sh in spec if (n, sh) not in qspec]
         self.spec = spec
         self.offsets: Dict[str, tuple] = {}
         off = 0
@@ -91,6 +129,21 @@ class ShardParams:
             self.v["head"] = self.v["embed"]
             if with_grad:
                 self.g["head"] = self.g["embed"]
+        self.s: Dict[str, torch.Tensor] = {}
+        self.q8 = self.scales = self.deq = None
+        if qspec:
+            qoff, soff, at = 0, 0, {}
+            for name, (N, K) in qspec:
+                at[name] = (qoff, soff, N, K)
+                qoff += (N * K + 255) // 256 * 256
+                soff += (N * (K // F8.BLOCK) + 63) // 64 * 64
+            self.q8 = torch.zeros(qoff, dtype=torch.float8_e4m3fn, device=self.device)
+            self.scales = torch.zeros(soff, dtype=torch.float32, device=self.device)
+            for name, (qo, so, N, K) in at.items():
+                self.v[name] = self.q8[qo:qo + N * K].view(N, K)
+                self.s[name] = self.scales[so:so + N * (K // F8.BLOCK)].view(N, K // F8.BLOCK)
+            # the GEMM paths' bf16 copy of one Linear at a time (dequant_fp8), sized for the largest
+            self.deq = torch.empty(max(N * K for _, (N, K) in qspec), dtype=torch.bfloat16, device=self.device)
 
     # ---- HF state dict  <->  fused layout ------------------------------------------------------------
     def load_hf_state_dict(self, sd: Dict[str, torch.Tensor]):
@@ -104,19 +157,23 @@ class ShardParams:
         for li in self.layer_ids:
             p = f"model.layers.{li}."
             put(f"l{li}.ln1", sd[p + "input_layernorm.weight"])
-            put(f"l{li}.wqkv", torch.cat([sd[p + "self_attn.q_proj.weight"], sd[p + "self_attn.k_proj.weight"],
-                                          sd[p + "self_attn.v_proj.weight"]], dim=0))
+            if self.fp8:
+                self._load_linears_fp8(sd, li)
+            else:
+                put(f"l{li}.wqkv", torch.cat([sd[p + "self_attn.q_proj.weight"], sd[p + "self_attn.k_proj.weight"],
+                                              sd[p + "self_attn.v_proj.weight"]], dim=0))
             if cfg.qkv_bias:
                 put(f"l{li}.bqkv", torch.cat([sd[p + "self_attn.q_proj.bias"], sd[p + "self_attn.k_proj.bias"],
                                               sd[p + "self_attn.v_proj.bias"]], dim=0))
             if cfg.qk_norm:
                 put(f"l{li}.qn", sd[p + "self_attn.q_norm.weight"])
                 put(f"l{li}.kn", sd[p + "self_attn.k_norm.weight"])
-            put(f"l{li}.wo", sd[p + "self_attn.o_proj.weight"])
             put(f"l{li}.ln2", sd[p + "post_attention_layernorm.weight"])
-            g, u = sd[p + "mlp.gate_proj.weight"], sd[p + "mlp.up_proj.weight"]
-            put(f"l{li}.wgu", torch.stack([g, u], dim=1).reshape(2 * cfg.intermediate, cfg.hidden))
-            put(f"l{li}.wd", sd[p + "mlp.down_proj.weight"])
+            if not self.fp8:
+                put(f"l{li}.wo", sd[p + "self_attn.o_proj.weight"])
+                g, u = sd[p + "mlp.gate_proj.weight"], sd[p + "mlp.up_proj.weight"]
+                put(f"l{li}.wgu", torch.stack([g, u], dim=1).reshape(2 * cfg.intermediate, cfg.hidden))
+                put(f"l{li}.wd", sd[p + "mlp.down_proj.weight"])
         if self.has_embed:
             put("embed", sd["model.embed_tokens.weight"])
         if self.has_head:
@@ -125,7 +182,8 @@ class ShardParams:
                 put("head", sd["lm_head.weight"] if "lm_head.weight" in sd else sd["model.embed_tokens.weight"])
 
     def hf_state_dict(self, grads: bool = False) -> Dict[str, torch.Tensor]:
-        """Inverse mapping (the role of ``parameters(distributed=True)``, module.py:577-650)."""
+        """Inverse mapping (the role of ``parameters(distributed=True)``, module.py:577-650).  An FP8 shard returns HF's
+        quantized names: ``...weight`` as float8_e4m3fn and ``...weight_scale_inv`` as the fp32 [N/128, K/128] grid."""
         cfg = self.cfg
         if grads and getattr(self, "grad_settle", None) is not None:
             self.grad_settle()          # matrix gradients are zeroed lazily after zero_grad() (ml/train.py)
@@ -155,7 +213,50 @@ class ShardParams:
             out["model.norm.weight"] = src["norm"].clone()
             # tied heads appear under both names, like HF's own state_dict()
             out["lm_head.weight"] = out["model.embed_tokens.weight"] if (cfg.tied and self.has_embed) else src["head"].clone()
-        return out
+        return self._with_scale_grids(out) if self.fp8 else out
+
+    def _load_linears_fp8(self, sd, li: int):
+        """Layer li's four Linears from HF's FP8 weight + scale_inv grid of each projection (a bf16 weight is quantized
+        first, by HF's rule), fused like the bf16 arena: q/k/v concatenated, gate/up row-interleaved."""
+        p = f"model.layers.{li}."
+        for name, projs in (("wqkv", ("self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj")),
+                            ("wo", ("self_attn.o_proj",)), ("wgu", ("mlp.gate_proj", "mlp.up_proj")),
+                            ("wd", ("mlp.down_proj",))):
+            qs, rs = [], []
+            for pre in (p + j for j in projs):
+                w = sd[pre + ".weight"]
+                if w.dtype == torch.float8_e4m3fn:
+                    q, inv = w.to(self.device), sd[pre + ".weight_scale_inv"].to(self.device)
+                else:
+                    q, inv = F8.quantize(w.to(self.device))
+                if tuple(inv.shape) != (q.shape[0] // F8.BLOCK, q.shape[1] // F8.BLOCK):
+                    raise NotImplementedError(f"{pre}.weight_scale_inv of shape {tuple(inv.shape)} for a weight of "
+                                              f"{tuple(q.shape)}: only 128x128 blocks are supported")
+                qs.append(q)
+                rs.append(F8.rows_from_grid(inv))
+            cat = (lambda ts: torch.stack(ts, dim=1).flatten(0, 1)) if name == "wgu" else (lambda ts: torch.cat(ts, dim=0))
+            self.v[f"l{li}.{name}"].copy_(cat(qs))
+            self.s[f"l{li}.{name}"].copy_(cat(rs))
+
+    def _with_scale_grids(self, out: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """``out`` with each FP8 ``...weight`` followed by its ``...weight_scale_inv`` grid, recovered from the rows."""
+        cfg, grids = self.cfg, {}
+        for li in self.layer_ids:
+            p = f"model.layers.{li}."
+            for pre, r in zip(("q_proj", "k_proj", "v_proj"),
+                              self.s[f"l{li}.wqkv"].split([cfg.q_dim, cfg.kv_dim, cfg.kv_dim], dim=0)):
+                grids[p + "self_attn." + pre] = r
+            grids[p + "self_attn.o_proj"] = self.s[f"l{li}.wo"]
+            sgu = self.s[f"l{li}.wgu"].view(cfg.intermediate, 2, -1)
+            grids[p + "mlp.gate_proj"], grids[p + "mlp.up_proj"] = sgu[:, 0], sgu[:, 1]
+            grids[p + "mlp.down_proj"] = self.s[f"l{li}.wd"]
+        res: Dict[str, torch.Tensor] = {}
+        for k, t in out.items():
+            res[k] = t
+            pre = k[:-len(".weight")]
+            if k.endswith(".weight") and pre in grids:
+                res[pre + ".weight_scale_inv"] = F8.grid_from_rows(grids[pre])
+        return res
 
     def init_seeded(self, seed: int = 1234):
         """Same values the CPU oracle draws (weights.init_state_dict), materialised layer by layer."""
@@ -174,12 +275,22 @@ class ShardParams:
         sub.load_hf_state_dict(sd)
 
     def init_on_device(self, seed: int = 1234, std: float = 0.02):
-        """Random init drawn directly on the GPU (benchmarks at 7B/8B scale; not comparable with the oracle)."""
+        """Random init drawn directly on the GPU (benchmarks at 7B/8B scale; not comparable with the oracle).  An FP8
+        shard draws each Linear's bf16 projections the same way and quantizes them on the device."""
         g = torch.Generator(device=self.device).manual_seed(seed)
         self.flat.normal_(0.0, std, generator=g)
         for name in self.v:
             if name.endswith(("ln1", "ln2", "qn", "kn")) or name == "norm":
                 self.v[name].fill_(1.0)
+        if self.fp8:
+            cfg, H, I = self.cfg, self.cfg.hidden, self.cfg.intermediate
+            shapes = {"self_attn.q_proj": (cfg.q_dim, H), "self_attn.k_proj": (cfg.kv_dim, H),
+                      "self_attn.v_proj": (cfg.kv_dim, H), "self_attn.o_proj": (H, cfg.q_dim), "mlp.gate_proj": (I, H),
+                      "mlp.up_proj": (I, H), "mlp.down_proj": (H, I)}
+            for li in self.layer_ids:
+                sd = {f"model.layers.{li}.{k}.weight": torch.empty(shape, dtype=torch.bfloat16, device=self.device).normal_(
+                    0.0, std, generator=g) for k, shape in shapes.items()}
+                self._load_linears_fp8(sd, li)
 
 
 @dataclass
@@ -268,6 +379,24 @@ class CudaLayerGroup:
         self.kvlen_dev.fill_(past_len)
 
     # ------------------------------------------------------------------------------------------ layer bodies
+    def _gemv(self, x: torch.Tensor, name: str, **kw) -> torch.Tensor:
+        """The decode Linear ``name`` of the arena: the bf16 GEMV, or on an FP8 shard the FP8 GEMV over its scales."""
+        p = self.p
+        if p.fp8:
+            return nat.gemv_fp8(x, p.v[name], p.s[name], **kw)
+        return nat.gemv(x, p.v[name], **kw)
+
+    def _gemm(self, a: torch.Tensor, name: str, **kw) -> torch.Tensor:
+        """The GEMM Linear ``name``; an FP8 shard first dequantizes it into the shard's bf16 scratch (one Linear at a
+        time: the launches run in stream order)."""
+        p = self.p
+        w = nat.dequant_fp8(p.v[name], p.s[name], out=p.deq) if p.fp8 else p.v[name]
+        return nat.gemm(a, w, **kw)
+
+    def gemv_rows(self) -> int:
+        """Rows per step up to which decode and verify steps run the weight-streaming GEMVs."""
+        return fp8_gemv_rows(self.cfg) if self.p.fp8 else gemv_max_rows()
+
     def _kv_start(self):
         """The per-row key starts for the attention and RoPE launches, or None (every row starts at slot 0)."""
         return self.kv_start_dev if self.ragged else None
@@ -277,15 +406,15 @@ class CudaLayerGroup:
         cfg, v, li = self.cfg, self.p.v, self.layer_ids[j]
         ks = self._kv_start()
         nat.rmsnorm_fwd(x, v[f"l{li}.ln1"], cfg.rms_eps, out=w.h)
-        nat.gemm(w.h, v[f"l{li}.wqkv"], out=w.qkv, bias=v.get(f"l{li}.bqkv"))
+        self._gemm(w.h, f"l{li}.wqkv", out=w.qkv, bias=v.get(f"l{li}.bqkv"))
         nat.rope_kv_fwd(w.qkv, w.q, self.kc[j], self.vc[j], self.pos_dev, self.cos, self.sin, v.get(f"l{li}.qn"),
                         v.get(f"l{li}.kn"), cfg.rms_eps, S, cfg.n_heads, cfg.n_kv_heads, cfg.head_dim, kv_start=ks)
         nat.attn_prefill_fwd(w.q, self.kc[j], self.vc[j], w.attn, None, B, S, past_len, cfg.n_heads, cfg.n_kv_heads,
                              cfg.head_dim, self.scale, kv_start=ks)
-        nat.gemm(w.attn, v[f"l{li}.wo"], out=x, residual=x)
+        self._gemm(w.attn, f"l{li}.wo", out=x, residual=x)
         nat.rmsnorm_fwd(x, v[f"l{li}.ln2"], cfg.rms_eps, out=w.h)
-        nat.gemm(w.h, v[f"l{li}.wgu"], out=w.act, flags=nat.EPI_SWIGLU)
-        nat.gemm(w.act, v[f"l{li}.wd"], out=x, residual=x)
+        self._gemm(w.h, f"l{li}.wgu", out=w.act, flags=nat.EPI_SWIGLU)
+        self._gemm(w.act, f"l{li}.wd", out=x, residual=x)
 
     FUSED_DECODE_MAX_T = 2048
 
@@ -317,13 +446,13 @@ class CudaLayerGroup:
         else:
             after = self.weights_after_last_layer            # lm_head on the last stage, else layer 0 for the next slot
         ctr = self.gemv_ctr[j]
-        nat.gemv(x, v[f"l{li}.wqkv"], out=w.qkv, bias=v.get(f"l{li}.bqkv"), norm_w=v[f"l{li}.ln1"], eps=cfg.rms_eps,
-                 next_w=v[f"l{li}.wo"], counter=ctr[0])
+        self._gemv(x, f"l{li}.wqkv", out=w.qkv, bias=v.get(f"l{li}.bqkv"), norm_w=v[f"l{li}.ln1"], eps=cfg.rms_eps,
+                   next_w=v[f"l{li}.wo"], counter=ctr[0])
         attention(j, li, B, w)
-        nat.gemv(w.attn, v[f"l{li}.wo"], out=x, residual=x, next_w=v[f"l{li}.wgu"], counter=ctr[1])
-        nat.gemv(x, v[f"l{li}.wgu"], out=w.act, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, flags=nat.EPI_SWIGLU,
-                 next_w=v[f"l{li}.wd"], counter=ctr[2])
-        nat.gemv(w.act, v[f"l{li}.wd"], out=x if out is None else out, residual=x, next_w=after, counter=ctr[3])
+        self._gemv(w.attn, f"l{li}.wo", out=x, residual=x, next_w=v[f"l{li}.wgu"], counter=ctr[1])
+        self._gemv(x, f"l{li}.wgu", out=w.act, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, flags=nat.EPI_SWIGLU,
+                   next_w=v[f"l{li}.wd"], counter=ctr[2])
+        self._gemv(w.act, f"l{li}.wd", out=x if out is None else out, residual=x, next_w=after, counter=ctr[3])
 
     def _layer_decode_batched(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor] = None,
                               attention=None, ws: Optional[torch.Tensor] = None):
@@ -336,15 +465,15 @@ class CudaLayerGroup:
             ws = self.gemm_ws if B <= 128 else None
         if j == 0:
             nat.rmsnorm_fwd(x, v[f"l{li}.ln1"], cfg.rms_eps, out=w.h)
-        nat.gemm(w.h, v[f"l{li}.wqkv"], out=w.qkv, bias=v.get(f"l{li}.bqkv"), ws=ws)
+        self._gemm(w.h, f"l{li}.wqkv", out=w.qkv, bias=v.get(f"l{li}.bqkv"), ws=ws)
         (attention or self._decode_attention)(j, li, B, w)
-        nat.gemm(w.attn, v[f"l{li}.wo"], out=x, residual=x, ws=ws, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, h_out=w.h)
-        nat.gemm(w.h, v[f"l{li}.wgu"], out=w.act, flags=nat.EPI_SWIGLU, ws=ws)
+        self._gemm(w.attn, f"l{li}.wo", out=x, residual=x, ws=ws, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, h_out=w.h)
+        self._gemm(w.h, f"l{li}.wgu", out=w.act, flags=nat.EPI_SWIGLU, ws=ws)
         if j + 1 < self.num_layers:
-            nat.gemm(w.act, v[f"l{li}.wd"], out=x, residual=x, ws=ws, norm_w=v[f"l{self.layer_ids[j + 1]}.ln1"],
-                     eps=cfg.rms_eps, h_out=w.h)
+            self._gemm(w.act, f"l{li}.wd", out=x, residual=x, ws=ws, norm_w=v[f"l{self.layer_ids[j + 1]}.ln1"],
+                       eps=cfg.rms_eps, h_out=w.h)
         else:
-            nat.gemm(w.act, v[f"l{li}.wd"], out=x if out is None else out, residual=x, ws=ws)
+            self._gemm(w.act, f"l{li}.wd", out=x if out is None else out, residual=x, ws=ws)
 
     def prefill(self, hidden: torch.Tensor, past_len: int = 0, kv_start=None) -> torch.Tensor:
         """hidden [B,S,H] -> [B,S,H]; appends S positions to the KV cache starting at ``past_len``.
@@ -395,7 +524,7 @@ class CudaLayerGroup:
             return
         for j in range(self.num_layers):
             o = out if j == self.num_layers - 1 else None
-            if B <= gemv_max_rows():
+            if B <= self.gemv_rows():
                 self._layer_decode(j, x, B, w, o)
             else:
                 self._layer_decode_batched(j, x, B, w, o)
@@ -433,7 +562,7 @@ class CudaLayerGroup:
         b = self.vbufs
         w = ShardBuffers(b.x[:n], b.h[:n], b.qkv[:n], b.q[:n], b.attn[:n], b.act[:n])
         for j in range(self.num_layers):
-            if n <= gemv_max_rows():
+            if n <= self.gemv_rows():
                 self._layer_decode(j, x, n, w, attention=self._verify_attention)
             else:
                 self._layer_decode_batched(j, x, n, w, attention=self._verify_attention, ws=self.ver_gemm_ws)
@@ -446,8 +575,9 @@ class CudaLayerGroup:
         import os
         cfg = self.cfg
         # the chain's ATTN job has no per-row key start: a left-padded slot takes the per-kernel sequence
+        # the chain's GEMV jobs stream bf16 weights: an FP8 shard takes the per-kernel sequence
         return (os.environ.get("TL_DECODE_IMPL", "kernels") == "chain" and self.allow_chain and self.num_layers > 0
-                and not self.ragged
+                and not self.ragged and not self.p.fp8
                 and B <= min(4, gemv_max_rows()) and cfg.n_kv_heads * B <= 60 and cfg.n_heads // cfg.n_kv_heads <= 8
                 and cfg.head_dim in (64, 128))
 
@@ -512,7 +642,8 @@ class CudaLayerGroup:
         of layer j+1 run as ONE two-job chain launch (one software dependency instead of a launch boundary between a
         long and a short weight stream)."""
         import os
-        return os.environ.get("TL_DECODE_IMPL", "kernels") == "dq" and self.allow_chain and self.num_layers > 1 and B <= min(4, gemv_max_rows())
+        return (os.environ.get("TL_DECODE_IMPL", "kernels") == "dq" and self.allow_chain and self.num_layers > 1
+                and B <= min(4, gemv_max_rows()) and not self.p.fp8)
 
     def _decode_step_dq(self, x: torch.Tensor, B: int, out: Optional[torch.Tensor]):
         cfg, v = self.cfg, self.p.v

@@ -35,14 +35,17 @@ class CudaStage:
     def __init__(self, cfg: ShardModelConfig, layer_ids, has_embed: bool, has_head: bool, device,
                  max_batch: int, max_seq: int, n_slots: int = 1, training: bool = False,
                  state_dict: Optional[Dict[str, torch.Tensor]] = None, seed: int = 1234, init: str = "seeded",
-                 max_tokens: Optional[int] = None):
+                 max_tokens: Optional[int] = None, quantization: Optional[dict] = None):
+        """``quantization``: ml/fp8.parse_quantization_config's result for an FP8 model (weight-only FP8 decoder
+        Linears), None for bf16."""
         nat.require_device()
         self.cfg = cfg
         self.device = torch.device(device)
         self.has_embed, self.has_head = has_embed, has_head
         self.supports_training, self.trainer = bool(training), None
         self.supports_kv_start = True       # prefill(kv_start=...): left-padded batches run as one batch
-        self.params = ShardParams(cfg, layer_ids, has_embed, has_head, self.device, with_grad=training)
+        self.params = ShardParams(cfg, layer_ids, has_embed, has_head, self.device, with_grad=training,
+                                  fp8=quantization is not None)
         if state_dict is not None:
             self.params.load_hf_state_dict(state_dict)
         elif init == "device":
@@ -469,7 +472,7 @@ class CudaStage:
     def n_decode_launches(self, B: int, ring: bool = False) -> int:
         """Kernel launches inside one decode step of this stage (for bench.py's gpu_launches claim)."""
         fused = self.slots[0].T_max <= self.slots[0].FUSED_DECODE_MAX_T
-        gemv = B <= gemv_max_rows()
+        gemv = B <= self.slots[0].gemv_rows()
         if self.slots[0].chain_ok(B):
             n = self.slots[0].n_chain_launches() + 2       # qkv of the first layer + one persistent launch per layer group
         elif self.slots[0].dq_ok(B):
@@ -478,6 +481,8 @@ class CudaStage:
         else:
             # GEMV path: 4 Linears + attention (1 fused / 3); batched: 4 GEMMs + 3 split-K reduce(+norm) passes + attention
             n = len(self.slots[0].layer_ids) * ((7 if gemv else 10) - (2 if fused else 0)) + 2 + (0 if gemv else 1)
+            if self.params.fp8:      # a second FP8 GEMV pass above 4 rows; the GEMM path dequantizes each Linear first
+                n += len(self.slots[0].layer_ids) * 4 * ((B > 4) if gemv else 1)
         if ring:
             n += (3 if self.has_embed else 2) - 2    # wait (+ token log) + signal, which also do the two position updates
         if self.has_embed:

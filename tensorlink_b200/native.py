@@ -41,6 +41,11 @@ _SIGS = {
                                 c_float, c_int, c_void_p, c_size_t, c_void_p]),
     "tl_gemv_bf16_ctr": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                  c_float, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "tl_gemv_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                            c_float, c_int, c_void_p]),
+    "tl_gemv_fp8_ctr": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                c_void_p, c_float, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "tl_dequant_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "tl_rope_table": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "tl_rope_kv_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_float, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -305,6 +310,53 @@ def gemv(x: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None, *
     nb = min(next_w.numel() * next_w.element_size(), prefetch_bytes()) if next_w is not None else 0
     _check(load().tl_gemv_bf16_ctr(_p(x), _p(w), _p(out), M, N, K, _p(bias), _p(residual), _p(norm_w), eps, flags,
                                    _p(counter), _p(next_w) if nb else None, nb, _stream()), "tl_gemv_bf16_ctr")
+    return out
+
+
+FP8_BLOCK = 128          # TL_FP8_BLOCK: columns per FP8 weight scale
+
+
+def _fp8(w: torch.Tensor, scales: torch.Tensor):
+    N, K = w.shape
+    assert w.dtype == torch.float8_e4m3fn and w.is_contiguous(), (w.dtype, w.is_contiguous())
+    assert scales.dtype == torch.float32 and scales.is_contiguous() and tuple(scales.shape) == (N, K // FP8_BLOCK), \
+        (scales.dtype, tuple(scales.shape), (N, K // FP8_BLOCK))
+    return N, K
+
+
+def gemv_fp8(x: torch.Tensor, w: torch.Tensor, scales: torch.Tensor, out: Optional[torch.Tensor] = None, *, bias=None,
+             residual=None, norm_w=None, eps: float = 1e-6, flags: int = 0, next_w: Optional[torch.Tensor] = None,
+             counter: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``gemv`` over FP8 weights ``w`` [N,K] (float8_e4m3fn) with ``scales`` [N, K/128] fp32: the weight used is
+    bf16(float(w) * scale), and the result equals ``gemv`` over ``dequant_fp8(w, scales)`` bit for bit."""
+    require_device()
+    _bf16(x, bias, residual, norm_w, out)
+    N, K = _fp8(w, scales)
+    M = x.shape[0]
+    assert x.shape[1] == K, (tuple(x.shape), K)
+    if out is None:
+        out = torch.empty(M, N // 2 if flags & EPI_SWIGLU else N, dtype=torch.bfloat16, device=x.device)
+    if bias is not None:
+        flags |= EPI_BIAS
+    if residual is not None:
+        flags |= EPI_RESIDUAL
+    nb = min(next_w.numel() * next_w.element_size(), prefetch_bytes()) if next_w is not None else 0
+    _check(load().tl_gemv_fp8_ctr(_p(x), _p(w), _p(scales), _p(out), M, N, K, _p(bias), _p(residual), _p(norm_w), eps,
+                                  flags, _p(counter), _p(next_w) if nb else None, nb, _stream()), "tl_gemv_fp8_ctr")
+    return out
+
+
+def dequant_fp8(w: torch.Tensor, scales: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """bf16 [N,K] = bf16(float(w) * scales[n][k/128]): HF's Fp8Dequantize followed by the cast to bf16.  ``out`` may be a
+    larger scratch buffer: its first N*K elements are written and returned as [N,K]."""
+    require_device()
+    N, K = _fp8(w, scales)
+    if out is None:
+        out = torch.empty(N, K, dtype=torch.bfloat16, device=w.device)
+    else:
+        assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() >= N * K
+        out = out.reshape(-1)[:N * K].view(N, K)
+    _check(load().tl_dequant_fp8(_p(w), _p(scales), _p(out), N, K, _stream()), "tl_dequant_fp8")
     return out
 
 
