@@ -203,6 +203,18 @@ int tl_lmhead_argmax(const void* x, const void* W, const void* norm_w, float eps
 /* argmax over bf16 logits[M,V] (any M); workspace >= M*64*8 bytes */
 int tl_argmax_bf16(const void* logits, int64_t* ids_out, void* workspace, size_t ws_bytes, int M, int V, void* stream);
 
+/* ---- the score log of generate(output_scores / output_logits): the _log twins of tl_argmax_bf16, tl_argmax_proc,
+ * tl_sample and tl_sample_proc pick the same ids (same draws, counters and histories) and also store each row into column
+ * c = log_col[0] of fp32 logs [n_cols, B_total, V] (column stride B_total*V, 64-bit offsets), launch row m at log row
+ * row0 + m: raw_log = float(bf16 logit); score_log = HF's score: the processed value (the logit itself without logits
+ * processors) for the argmax, and x / temperature (IEEE division) on the sampler's kept set, -inf elsewhere, for the
+ * samplers (x: the processed value for tl_sample_proc_log).  Either log may be NULL, not both.  log_col: int32[2] in
+ * device memory, {column, exit word}; the exit word must be 0 and is left 0.  The call advances the column by one, so a
+ * captured graph logs each replay into the next column; a column >= n_cols is not written.  A NULL log_col, row0 + M >
+ * B_total, or n_cols*B_total*V beyond int64 is rejected (TL_ERR_INVALID).  No launch is added. */
+int tl_argmax_bf16_log(const void* logits, int64_t* ids_out, void* workspace, size_t ws_bytes, int M, int V, float* raw_log,
+                       float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream);
+
 /* ---- token sampling on the device (csrc/sample.cu): what HF `generate(do_sample=True)` does on the host's copy of the
  * logits (the reference delegates to it, tensorlink/ml/module.py:763-769, ml/worker.py:403-404): temperature -> top-k
  * (every logit >= the k-th largest is kept; 0 = off) -> top-p (a token is kept while the probability mass above it is
@@ -212,6 +224,9 @@ int tl_argmax_bf16(const void* logits, int64_t* ids_out, void* workspace, size_t
 size_t tl_sample_ws(int M);
 int tl_sample(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
               unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream);
+int tl_sample_log(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
+                  unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, float* raw_log,
+                  float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream);
 /* speculative sampling after a verify pass (Leviathan et al. Algorithm 1, HF _speculative_sampling), one row: the
  * target's rows p_logits bf16 [K+1, V_p] and the assistant's q_logits bf16 [K, V_q], each warped by tl_sample's rules
  * with the same temperature / top_k / top_p; the drafts d_i = in_ids[i+1] for i < n = min(*n_cand, K).  Draft i is kept
@@ -255,6 +270,14 @@ int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* 
 int tl_sample_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
                    const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
                    unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream);
+/* the score-log twins (see tl_argmax_bf16_log) */
+int tl_argmax_proc_log(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                       const int32_t* params_dev, int flags, void* workspace, size_t ws_bytes, int M, int V, int L,
+                       float* raw_log, float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream);
+int tl_sample_proc_log(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                       const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
+                       unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, float* raw_log,
+                       float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream);
 
 /* ---- prompt-lookup decoding (csrc/prompt_lookup.cu), one row: a verify step runs in_ids[0..K] (the last history token
  * and K drafts) as K+1 rows and keeps the drafts the model agrees with.  The history is the logits processors' (log, len,

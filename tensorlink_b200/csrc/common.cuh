@@ -89,6 +89,40 @@ __device__ __forceinline__ void lp_append(const LpRows& h, int m, int id) {
 // ids while below min_new_tokens
 int lp_ban_launch(const LpRows& h, uint32_t* ban, int M, int V, cudaStream_t stream);
 
+// ---------------------------------------------------------------- score log (generate's output_scores / output_logits)
+// The picking kernels of a decode step (the argmax, the samplers) also store each row's values into column c of fp32
+// logs [n_cols, B_total, V]: raw = float(bf16 logit) and proc = the score HF returns (processed, warped).  c is read from
+// device memory and the step's last kernel advances it, so a captured graph writes every replay into the next column.
+struct LogDesc {
+    float* raw;                 // or nullptr
+    float* proc;                // or nullptr
+    int32_t* col;               // {column, exit word}: the exit word is zero between launches (last_cta_out)
+    long long col_stride;       // B_total * V
+    int row0, n_cols;           // row m of the launch is log row row0 + m; columns >= n_cols are not written
+    float temperature;          // the samplers' score of a kept value x: x / temperature (IEEE division, as HF)
+};
+// the log rows of launch row m in column c, or false when c lies outside the log
+__device__ __forceinline__ bool log_rows(const LogDesc& d, int c, int m, int V, float** raw, float** proc) {
+    if (c < 0 || c >= d.n_cols) return false;
+    const long long off = (long long)c * d.col_stride + (long long)(d.row0 + m) * V;
+    *raw = d.raw ? d.raw + off : nullptr;
+    *proc = d.proc ? d.proc + off : nullptr;
+    return true;
+}
+// checks a log's arguments for M rows of V values and fills *d (the host half of every _log entry point)
+inline int make_log(const char* who, float* raw, float* proc, int32_t* col, int n_cols, int B_total, int row0, int M, int V,
+                    float temperature, LogDesc* d) {
+    TL_REQUIRE(col, TL_ERR_INVALID, "%s: null column counter", who);
+    TL_REQUIRE(raw || proc, TL_ERR_INVALID, "%s: neither a raw nor a score log", who);
+    TL_REQUIRE(n_cols >= 1 && row0 >= 0 && M >= 0 && V >= 1 && (long long)row0 + M <= B_total, TL_ERR_INVALID,
+               "%s: bad log shape n_cols=%d B_total=%d row0=%d M=%d", who, n_cols, B_total, row0, M);
+    const long long stride = (long long)B_total * V;
+    TL_REQUIRE(stride <= (long long)(~0ull >> 1) / n_cols, TL_ERR_INVALID, "%s: a log of %d x %d x %d values overflows",
+               who, n_cols, B_total, V);
+    *d = LogDesc{raw, proc, col, stride, row0, n_cols, temperature};
+    return TL_OK;
+}
+
 // ---------------------------------------------------------------- mbarrier / TMA PTX
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));

@@ -3,15 +3,17 @@
 // two-stage argmax picks the lowest index among equal maxima, which is what torch.argmax returns.
 // With PROC the argmax runs over HF's processed values (repetition penalty, ban set: logits_process.cu), computed in
 // fp32 as each logit is read, and the final stage appends the picked id to the row's history.
+// With LOG the part kernel also stores every value it reads into the score log (common.cuh LogDesc): nothing else reads
+// the row again.
 #include "common.cuh"
 
 namespace tl {
 
 constexpr int AM_PARTS = 64, AM_THREADS = 256;
 
-template <bool PROC>
+template <bool PROC, bool LOG = false>
 __global__ void __launch_bounds__(AM_THREADS) argmax_part_kernel(const bf16* __restrict__ logits, float* __restrict__ pval,
-                                                                 int* __restrict__ pidx, int V, LpRows h) {
+                                                                 int* __restrict__ pidx, int V, LpRows h, LogDesc lg) {
     const int m = blockIdx.y, part = blockIdx.x;
     const int per = (V + AM_PARTS - 1) / AM_PARTS;
     const int lo = part * per, hi = min(V, lo + per);
@@ -19,11 +21,18 @@ __global__ void __launch_bounds__(AM_THREADS) argmax_part_kernel(const bf16* __r
     const uint32_t* bits = PROC ? h.bits + (size_t)m * h.W : nullptr;
     const uint32_t* ban = PROC && h.ban ? h.ban + (size_t)m * h.W : nullptr;
     const float penalty = PROC ? __int_as_float(h.params[TL_LP_PENALTY]) : 1.f;
+    float *raw = nullptr, *proc = nullptr;
+    const bool log = LOG && log_rows(lg, *lg.col, m, V, &raw, &proc);
     float best = -INFINITY;
     int bi = 0x7fffffff;
     for (int i = lo + threadIdx.x; i < hi; i += AM_THREADS) {
-        float v = bf2f(row[i]);
+        const float x = bf2f(row[i]);
+        float v = x;
         if (PROC) v = lp_value(v, i, bits, ban, penalty);
+        if (LOG && log) {                       // greedy: the score is the processed value (the logit itself without PROC)
+            if (raw) raw[i] = x;
+            if (proc) proc[i] = v;
+        }
         if (v > best) { best = v; bi = i; }     // ascending i per thread: first max kept
     }
 #pragma unroll
@@ -44,9 +53,10 @@ __global__ void __launch_bounds__(AM_THREADS) argmax_part_kernel(const bf16* __r
     }
 }
 
-template <bool PROC>
+// LOG: the step's last kernel advances the log column, after every part kernel read it (stream order)
+template <bool PROC, bool LOG = false>
 __global__ void argmax_final_kernel(const float* __restrict__ pval, const int* __restrict__ pidx,
-                                    int64_t* __restrict__ ids_out, LpRows h) {
+                                    int64_t* __restrict__ ids_out, LpRows h, int32_t* __restrict__ log_col) {
     const int m = blockIdx.x, lane = threadIdx.x;
     float best = -INFINITY;
     int bi = 0x7fffffff;
@@ -65,6 +75,7 @@ __global__ void argmax_final_kernel(const float* __restrict__ pval, const int* _
         const int id = (bi == 0x7fffffff) ? 0 : bi;
         ids_out[m] = (int64_t)id;
         if (PROC) lp_append(h, m, id);
+        if (LOG && m == 0) log_col[0] += 1;
     }
 }
 
@@ -76,7 +87,8 @@ size_t tl_lmhead_ws(int M, int V) {
     return (size_t)M * V * sizeof(tl::bf16) + (size_t)M * tl::AM_PARTS * (sizeof(float) + sizeof(int)) + 256;
 }
 
-int tl_argmax_bf16(const void* logits, int64_t* ids_out, void* workspace, size_t ws_bytes, int M, int V, void* stream) {
+static int argmax_launch(const void* logits, int64_t* ids_out, void* workspace, size_t ws_bytes, int M, int V, const tl::LogDesc* lg,
+                         void* stream) {
     using namespace tl;
     const size_t need = (size_t)M * AM_PARTS * (sizeof(float) + sizeof(int));
     TL_REQUIRE(ws_bytes >= need, TL_ERR_WORKSPACE, "tl_argmax_bf16: workspace %zu < %zu", ws_bytes, need);
@@ -84,13 +96,33 @@ int tl_argmax_bf16(const void* logits, int64_t* ids_out, void* workspace, size_t
     float* pval = (float*)workspace;
     int* pidx = (int*)(pval + (size_t)M * AM_PARTS);
     cudaStream_t st = (cudaStream_t)stream;
-    argmax_part_kernel<false><<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V, LpRows{});
-    argmax_final_kernel<false><<<M, 32, 0, st>>>(pval, pidx, ids_out, LpRows{});
+    if (lg) {
+        argmax_part_kernel<false, true><<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V, LpRows{}, *lg);
+        argmax_final_kernel<false, true><<<M, 32, 0, st>>>(pval, pidx, ids_out, LpRows{}, lg->col);
+    } else {
+        argmax_part_kernel<false><<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V, LpRows{}, LogDesc{});
+        argmax_final_kernel<false><<<M, 32, 0, st>>>(pval, pidx, ids_out, LpRows{}, nullptr);
+    }
     return check_launch("tl_argmax_bf16");
 }
 
-int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
-                   const int32_t* params_dev, int flags, void* workspace, size_t ws_bytes, int M, int V, int L, void* stream) {
+int tl_argmax_bf16(const void* logits, int64_t* ids_out, void* workspace, size_t ws_bytes, int M, int V, void* stream) {
+    return argmax_launch(logits, ids_out, workspace, ws_bytes, M, V, nullptr, stream);
+}
+
+int tl_argmax_bf16_log(const void* logits, int64_t* ids_out, void* workspace, size_t ws_bytes, int M, int V, float* raw_log,
+                       float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream) {
+    using namespace tl;
+    TL_REQUIRE(logits && ids_out && workspace, TL_ERR_INVALID, "tl_argmax_bf16_log: null argument");
+    LogDesc lg;
+    const int rc = make_log("tl_argmax_bf16_log", raw_log, score_log, log_col, n_cols, B_total, row0, M, V, 1.f, &lg);
+    if (rc != TL_OK) return rc;
+    return argmax_launch(logits, ids_out, workspace, ws_bytes, M, V, &lg, stream);
+}
+
+static int argmax_proc_launch(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                              const int32_t* params_dev, int flags, void* workspace, size_t ws_bytes, int M, int V, int L,
+                              const tl::LogDesc* lg, void* stream) {
     using namespace tl;
     TL_REQUIRE(logits && ids_out && log && len && bits && params_dev && workspace, TL_ERR_INVALID, "tl_argmax_proc: null argument");
     TL_REQUIRE(M >= 1 && V >= 1 && L >= 1, TL_ERR_INVALID, "tl_argmax_proc: bad shape M=%d V=%d L=%d", M, V, L);
@@ -105,9 +137,29 @@ int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* 
         const int rc = lp_ban_launch(h, ban, M, V, st);
         if (rc != TL_OK) return rc;
     }
-    argmax_part_kernel<true><<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V, h);
-    argmax_final_kernel<true><<<M, 32, 0, st>>>(pval, pidx, ids_out, h);
+    if (lg) {
+        argmax_part_kernel<true, true><<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V, h, *lg);
+        argmax_final_kernel<true, true><<<M, 32, 0, st>>>(pval, pidx, ids_out, h, lg->col);
+    } else {
+        argmax_part_kernel<true><<<dim3(AM_PARTS, M), AM_THREADS, 0, st>>>((const bf16*)logits, pval, pidx, V, h, LogDesc{});
+        argmax_final_kernel<true><<<M, 32, 0, st>>>(pval, pidx, ids_out, h, nullptr);
+    }
     return check_launch("tl_argmax_proc");
+}
+
+int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                   const int32_t* params_dev, int flags, void* workspace, size_t ws_bytes, int M, int V, int L, void* stream) {
+    return argmax_proc_launch(logits, ids_out, log, len, bits, params_dev, flags, workspace, ws_bytes, M, V, L, nullptr, stream);
+}
+
+int tl_argmax_proc_log(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                       const int32_t* params_dev, int flags, void* workspace, size_t ws_bytes, int M, int V, int L,
+                       float* raw_log, float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream) {
+    using namespace tl;
+    LogDesc lg;
+    const int rc = make_log("tl_argmax_proc_log", raw_log, score_log, log_col, n_cols, B_total, row0, M, V, 1.f, &lg);
+    if (rc != TL_OK) return rc;
+    return argmax_proc_launch(logits, ids_out, log, len, bits, params_dev, flags, workspace, ws_bytes, M, V, L, &lg, stream);
 }
 
 int tl_lmhead_argmax(const void* x, const void* W, const void* norm_w, float eps, int64_t* ids_out, void* logits_out,

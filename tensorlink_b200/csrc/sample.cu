@@ -158,9 +158,15 @@ __device__ __forceinline__ RowStats row_analysis(const uint16_t* __restrict__ lr
     return RowStats{x_max, p_key, Z_kept};
 }
 
+// LOG: once p_key is known, a pass over the row stores it into the score log (common.cuh LogDesc): the raw logit, and
+// x / temperature on the kept set, -inf elsewhere.  The pass strides by the CTA's width, so its stores coalesce (the
+// draw's per-thread ranges would scatter them).  The CTAs (rows) share the log column, so the last CTA out advances it.
+// The draw itself does not depend on LOG.
+template <bool LOG = false>
 __global__ void __launch_bounds__(SM_THREADS) sample_kernel(const bf16* __restrict__ logits, int64_t* __restrict__ ids_out, int V,
                                                             float inv_temp, int top_k, float top_p, unsigned long long seed,
-                                                            int32_t* __restrict__ counters, uint32_t* __restrict__ hist_all) {
+                                                            int32_t* __restrict__ counters, uint32_t* __restrict__ hist_all,
+                                                            LogDesc lg) {
     const int row = blockIdx.x, tid = threadIdx.x;
     const uint16_t* lr = reinterpret_cast<const uint16_t*>(logits) + (size_t)row * V;
     __shared__ double s_warp[32];
@@ -173,6 +179,14 @@ __global__ void __launch_bounds__(SM_THREADS) sample_kernel(const bf16* __restri
     const double target = (double)philox_uniform(seed, (uint32_t)row, ctr) * Z_kept;
     const int per = (V + SM_THREADS - 1) / SM_THREADS;
     const int i0 = tid * per, i1 = min(V, i0 + per);
+    float *raw = nullptr, *proc = nullptr;
+    if (LOG && log_rows(lg, *lg.col, row, V, &raw, &proc)) {
+        for (int i = tid; i < V; i += SM_THREADS) {          // interleaved, not the draw's per-thread ranges: coalesced stores
+            const float x = __uint_as_float((uint32_t)lr[i] << 16);
+            if (raw) raw[i] = x;
+            if (proc) proc[i] = (int)bf16_key(lr[i]) >= p_key ? __fdiv_rn(x, lg.temperature) : -INFINITY;
+        }
+    }
     double local_w = 0.0;
     for (int i = i0; i < i1; ++i) {
         const uint32_t key = bf16_key(lr[i]);
@@ -203,6 +217,10 @@ __global__ void __launch_bounds__(SM_THREADS) sample_kernel(const bf16* __restri
         }
         ids_out[row] = (int64_t)pick;
         counters[row] = (int32_t)(ctr + 1u);
+        if (LOG && last_cta_out((unsigned*)lg.col + 1)) {
+            lg.col[0] += 1;
+            __threadfence();
+        }
     }
 }
 
@@ -396,10 +414,12 @@ __device__ __forceinline__ void clear_bins(u64* h) {
     __syncthreads();
 }
 
+// LOG: as sample_kernel's, over the processed values (-inf for a banned id stays -inf)
+template <bool LOG = false>
 __global__ void __launch_bounds__(SM_THREADS) sample_proc_kernel(const bf16* __restrict__ logits, int64_t* __restrict__ ids_out,
                                                                  int V, LpRows h, float inv_temp, int top_k, float top_p,
                                                                  unsigned long long seed, int32_t* __restrict__ counters,
-                                                                 u64* __restrict__ hist_all) {
+                                                                 u64* __restrict__ hist_all, LogDesc lg) {
     const int row = blockIdx.x, tid = threadIdx.x;
     const bf16* lr = logits + (size_t)row * V;
     const uint32_t* bits = h.bits + (size_t)row * h.W;
@@ -425,11 +445,24 @@ __global__ void __launch_bounds__(SM_THREADS) sample_proc_kernel(const bf16* __r
     __syncthreads();
     vmax = warp_max(s_max[tid & 31]);
     const uint32_t ctr = (uint32_t)counters[row];
+    float *raw = nullptr, *proc = nullptr;
+    const bool log = LOG && log_rows(lg, *lg.col, row, V, &raw, &proc);
     if (vmax == -INFINITY) {                  // every token banned: token 0, as the argmax returns
+        if (LOG && log) {
+            for (int i = tid; i < V; i += SM_THREADS) {
+                if (raw) raw[i] = bf2f(lr[i]);
+                if (proc) proc[i] = -INFINITY;
+            }
+        }
+        if (LOG) __syncthreads();
         if (tid == 0) {
             ids_out[row] = 0;
             counters[row] = (int32_t)(ctr + 1u);
             lp_append(h, row, 0);
+            if (LOG && last_cta_out((unsigned*)lg.col + 1)) {
+                lg.col[0] += 1;
+                __threadfence();
+            }
         }
         return;
     }
@@ -469,6 +502,13 @@ __global__ void __launch_bounds__(SM_THREADS) sample_proc_kernel(const bf16* __r
     // ---- draw and invert the CDF over the kept tokens in index order (integer prefix sums: exact)
     const int per = (V + SM_THREADS - 1) / SM_THREADS;
     const int i0 = tid * per, i1 = min(V, i0 + per);
+    if (LOG && log) {
+        for (int i = tid; i < V; i += SM_THREADS) {          // interleaved, not the draw's per-thread ranges: coalesced stores
+            const float x = bf2f(lr[i]), v = lp_value(x, i, bits, ban, penalty);
+            if (raw) raw[i] = x;
+            if (proc) proc[i] = f32_key(v) >= p_key ? __fdiv_rn(v, lg.temperature) : -INFINITY;
+        }
+    }
     u64 local_w = 0;
     for (int i = i0; i < i1; ++i) {
         const uint32_t key = key_at(i);
@@ -493,6 +533,10 @@ __global__ void __launch_bounds__(SM_THREADS) sample_proc_kernel(const bf16* __r
         ids_out[row] = (int64_t)pick;
         counters[row] = (int32_t)(ctr + 1u);
         lp_append(h, row, pick);
+        if (LOG && last_cta_out((unsigned*)lg.col + 1)) {
+            lg.col[0] += 1;
+            __threadfence();
+        }
     }
 }
 
@@ -500,9 +544,10 @@ __global__ void __launch_bounds__(SM_THREADS) sample_proc_kernel(const bf16* __r
 
 extern "C" {
 
-int tl_sample_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
-                   const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
-                   unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream) {
+static int sample_proc_launch(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                              const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
+                              unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes,
+                              const tl::LogDesc* lg, void* stream) {
     using namespace tl;
     TL_REQUIRE(logits && ids_out && log && len && bits && params_dev && counters_dev && workspace, TL_ERR_INVALID,
                "tl_sample_proc: null argument");
@@ -518,24 +563,68 @@ int tl_sample_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* 
         const int rc = lp_ban_launch(h, ban, M, V, st);
         if (rc != TL_OK) return rc;
     }
-    sample_proc_kernel<<<M, SM_THREADS, 0, st>>>((const bf16*)logits, ids_out, V, h, 1.0f / temperature, top_k, top_p, seed,
-                                                 counters_dev, (u64*)((unsigned char*)workspace + lp_ban_bytes(M, V)));
+    u64* hist = (u64*)((unsigned char*)workspace + lp_ban_bytes(M, V));
+    if (lg)
+        sample_proc_kernel<true><<<M, SM_THREADS, 0, st>>>((const bf16*)logits, ids_out, V, h, 1.0f / temperature, top_k, top_p, seed,
+                                                           counters_dev, hist, *lg);
+    else
+        sample_proc_kernel<<<M, SM_THREADS, 0, st>>>((const bf16*)logits, ids_out, V, h, 1.0f / temperature, top_k, top_p, seed,
+                                                     counters_dev, hist, LogDesc{});
     return check_launch("tl_sample_proc");
+}
+
+int tl_sample_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                   const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
+                   unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream) {
+    return sample_proc_launch(logits, ids_out, log, len, bits, params_dev, flags, M, V, L, temperature, top_k, top_p, seed,
+                              counters_dev, workspace, ws_bytes, nullptr, stream);
+}
+
+int tl_sample_proc_log(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
+                       const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
+                       unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, float* raw_log,
+                       float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream) {
+    using namespace tl;
+    LogDesc lg;
+    const int rc = make_log("tl_sample_proc_log", raw_log, score_log, log_col, n_cols, B_total, row0, M, V, temperature, &lg);
+    if (rc != TL_OK) return rc;
+    return sample_proc_launch(logits, ids_out, log, len, bits, params_dev, flags, M, V, L, temperature, top_k, top_p, seed,
+                              counters_dev, workspace, ws_bytes, &lg, stream);
 }
 
 size_t tl_sample_ws(int M) { return (size_t)(M > 0 ? M : 0) * tl::SM_BINS * sizeof(uint32_t); }
 
-int tl_sample(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
-              unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream) {
+static int sample_launch(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
+                         unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, const tl::LogDesc* lg,
+                         void* stream) {
     using namespace tl;
     TL_REQUIRE(logits && ids_out && counters_dev && workspace, TL_ERR_INVALID, "tl_sample: null argument");
     TL_REQUIRE(M >= 1 && V >= 1, TL_ERR_INVALID, "tl_sample: bad shape M=%d V=%d", M, V);
     TL_REQUIRE(temperature > 0.f && top_p > 0.f && top_p <= 1.f && top_k >= 0, TL_ERR_INVALID,
                "tl_sample: temperature must be > 0, 0 < top_p <= 1, top_k >= 0 (got %g, %g, %d)", temperature, top_p, top_k);
     TL_REQUIRE(ws_bytes >= tl_sample_ws(M), TL_ERR_INVALID, "tl_sample: workspace too small");
-    sample_kernel<<<M, SM_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, ids_out, V, 1.0f / temperature, top_k, top_p, seed,
-                                                              counters_dev, (uint32_t*)workspace);
+    if (lg)
+        sample_kernel<true><<<M, SM_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, ids_out, V, 1.0f / temperature, top_k,
+                                                                        top_p, seed, counters_dev, (uint32_t*)workspace, *lg);
+    else
+        sample_kernel<<<M, SM_THREADS, 0, (cudaStream_t)stream>>>((const bf16*)logits, ids_out, V, 1.0f / temperature, top_k, top_p,
+                                                                  seed, counters_dev, (uint32_t*)workspace, LogDesc{});
     return check_launch("tl_sample");
+}
+
+int tl_sample(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
+              unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream) {
+    return sample_launch(logits, ids_out, M, V, temperature, top_k, top_p, seed, counters_dev, workspace, ws_bytes, nullptr, stream);
+}
+
+int tl_sample_log(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
+                  unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, float* raw_log,
+                  float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream) {
+    using namespace tl;
+    LogDesc lg;
+    const int rc = make_log("tl_sample_log", raw_log, score_log, log_col, n_cols, B_total, row0, M, V, temperature, &lg);
+    if (rc != TL_OK) return rc;
+    return sample_launch(logits, ids_out, M, V, temperature, top_k, top_p, seed, counters_dev, workspace, ws_bytes, &lg, stream);
 }
 
 size_t tl_spec_accept_ws(int K) {

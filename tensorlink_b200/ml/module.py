@@ -247,6 +247,19 @@ def _left_pad_starts(mask: torch.Tensor):
 EOS_CHECK_EVERY = 16       # decode steps between two host-side "has every row emitted EOS?" checks
 
 
+def _output_flags(return_dict_in_generate=None, output_scores=None, output_logits=None) -> Optional[dict]:
+    """HF's ``return_dict_in_generate`` / ``output_scores`` / ``output_logits`` as {scores, logits} (what to log), or
+    None when the plain tensor is returned.  Each accepts True, False or None; without ``return_dict_in_generate=True``
+    the other two are ignored, as HF ignores them."""
+    for name, v in (("return_dict_in_generate", return_dict_in_generate), ("output_scores", output_scores),
+                    ("output_logits", output_logits)):
+        if v is not None and not isinstance(v, bool):
+            raise ValueError(f"{name} has to be True, False or None, but is {v!r}")
+    if not return_dict_in_generate:
+        return None
+    return {"scores": bool(output_scores), "logits": bool(output_logits)}
+
+
 def _eos_list(eos_token_id):
     if eos_token_id is None:
         return []
@@ -679,7 +692,22 @@ class DistributedModel(torch.nn.Module):
         agreement of 0.8 per draft token (not measured on real checkpoints); it changes speed only: never the greedy output,
         nor the distribution of the sampled one.
         ``num_assistant_tokens_schedule`` may only be "constant" and ``assistant_confidence_threshold`` only None.
-        ``self.timers["assisted_steps"]`` counts the verify steps."""
+        ``self.timers["assisted_steps"]`` counts the verify steps.
+        ``return_dict_in_generate=True`` returns HF's ``GenerateDecoderOnlyOutput`` (transformers is imported then only):
+        ``sequences`` is the tensor above; ``scores`` / ``logits`` (with ``output_scores`` / ``output_logits``, else None)
+        are tuples of fp32 [B, V] tensors on the stage's device, one per generated column.  ``logits[c][r]`` is
+        float(bf16 logit) of row r, the values that picked its token; ``scores[c][r]`` is HF's processed and warped row:
+        greedy, the logits after the logits processors (-inf for a banned id); sampled, x / temperature (IEEE fp32
+        division) on the sampler's kept set and -inf elsewhere, so the emitted token's score is always finite.  The last
+        stage's picking kernels log them inside the decode graph (no added launch) into buffers that cost
+        B * max_new_tokens * V * 4 bytes per kind (2.5 GB for 32 rows x 128 tokens x 152,064 ids); the returned tensors
+        are copies, broadcast from the last rank, and cut where the EOS check cuts ``sequences``.  ``attentions``,
+        ``hidden_states`` and ``past_key_values`` are None (HF returns its cache as ``past_key_values``).  After a row's
+        EOS its entries are this model's continuation of its own tokens, where HF feeds ``pad_token_id``.
+        Without ``return_dict_in_generate=True``, ``output_scores`` / ``output_logits`` are ignored, as in HF, and the call
+        runs exactly as without them.  With prompt lookup or an assistant, with the grouped left-padded path of a stage
+        without ``supports_kv_start``, or on a non-CUDA stage, ``return_dict_in_generate=True`` raises
+        NotImplementedError.  ``compute_transition_scores`` turns ``scores`` into per-token log-probabilities."""
         input_ids = kwargs.pop("input_ids", args[0] if args else None)
         max_new = int(kwargs.pop("max_new_tokens", 20))
         streamer = kwargs.pop("streamer", None)
@@ -701,11 +729,17 @@ class DistributedModel(torch.nn.Module):
         ngram = kwargs.pop("max_matching_ngram_size", None) if lookup is not None else None
         assistant = kwargs.pop("assistant_model", None)
         n_assist = kwargs.pop("num_assistant_tokens", None) if assistant is not None else None
+        out = _output_flags(kwargs.pop("return_dict_in_generate", None), kwargs.pop("output_scores", None),
+                            kwargs.pop("output_logits", None))
         _check_unconsumed(kwargs, "DistributedModel.generate")
         if assistant is not None and lookup is not None:
             # (HF drafts by prompt lookup here and ignores the assistant without a word)
             raise NotImplementedError("assistant_model together with prompt_lookup_num_tokens: pick one draft source")
+        if out is not None and (lookup is not None or assistant is not None):
+            raise NotImplementedError("return_dict_in_generate=True with prompt_lookup_num_tokens / assistant_model")
         link, st, cfg = self.link, self.stage, self.cfg
+        if out is not None and not hasattr(st, "set_score_log"):
+            raise NotImplementedError("return_dict_in_generate=True needs the CUDA stage")
         groups, padded = None, None
         if link.first and mask is not None:
             if tuple(mask.shape) != tuple(input_ids.shape):
@@ -737,24 +771,69 @@ class DistributedModel(torch.nn.Module):
             if procs is not None:                # the grouped runs would see each row's history without its pads
                 raise NotImplementedError("repetition_penalty / no_repeat_ngram_size / min_new_tokens with a left-padded "
                                           "batch need a stage with per-row key starts (supports_kv_start)")
+            if out is not None:                  # the grouped runs return their rows in separate calls
+                raise NotImplementedError("return_dict_in_generate=True with a left-padded batch needs a stage with "
+                                          "per-row key starts (supports_kv_start)")
             return self._generate_left_padded(input_ids, groups[0], groups[1], max_new, streamer, use_graph, sampling)
         if procs is not None and link.first:     # the starting history: every column, the dropped pad columns too
             procs["history"] = input_ids.cpu() if padded is None else torch.cat([padded[0], input_ids.cpu()], dim=1)
         result = self._generate_batch(input_ids, max_new, streamer, use_graph, profile, sampling, procs,
-                                      None if padded is None else padded[1])
+                                      None if padded is None else padded[1], **({} if out is None else {"out": out}))
+        if out is not None:
+            result, scores, logits = result
         if padded is not None and padded[0].shape[1]:
             result = torch.cat([padded[0].to(result.device), result], dim=1)
-        return result
+        if out is None:
+            return result
+        from transformers.generation import GenerateDecoderOnlyOutput
+        return GenerateDecoderOnlyOutput(sequences=result, scores=scores, logits=logits)
 
-    def _generate_batch(self, input_ids, max_new, streamer, use_graph, profile, sampling, procs, kv_start):
+    def compute_transition_scores(self, sequences: torch.Tensor, scores, normalize_logits: bool = False) -> torch.Tensor:
+        """HF ``compute_transition_scores`` without beams: [B, len(scores)] = each emitted token's score at its column,
+        log-softmax normalised over the vocabulary first with ``normalize_logits`` (per-token log-probabilities from
+        ``generate(..., return_dict_in_generate=True, output_scores=True)``; with ``do_sample`` they are those of the
+        warped distribution).  The generated columns are the last len(scores) of ``sequences``."""
+        T = len(scores)
+        stacked = torch.stack(scores).reshape(T, -1).transpose(0, 1)          # [B*V, T], HF's layout
+        V = scores[0].shape[-1]
+        if normalize_logits:
+            stacked = torch.nn.functional.log_softmax(stacked.reshape(-1, V, T), dim=1).reshape(-1, T)
+        rows = torch.arange(scores[0].shape[0], device=sequences.device).view(-1, 1) * V
+        return stacked.gather(0, sequences[:, sequences.shape[-1] - T:] + rows)
+
+    def _with_scores(self, result: torch.Tensor, S: int, out):
+        """``result`` of a finished run, or with ``out`` (``_output_flags``) (result, scores, logits): the last stage's
+        score log, columns 0..n_new-1 for the n_new generated columns ``result`` kept, on every rank; scores and logits
+        are each a tuple of n_new fp32 [B, V] tensors, or None when not asked for."""
+        if out is None:
+            return result
+        link, st = self.link, self.stage
+        B, n_new = result.shape[0], result.shape[1] - S
+        got = []
+        for kind in ("scores", "logits"):
+            if not out[kind]:
+                got.append(None)
+                continue
+            if link.last:
+                t = st.score_log_copy(kind, B, n_new)
+            else:
+                t = torch.empty(n_new, B, self.cfg.vocab, dtype=torch.float32, device=self.device)
+            link.broadcast(t, self.world - 1)
+            got.append(tuple(t.unbind(0)))
+        return (result, *got)
+
+    def _generate_batch(self, input_ids, max_new, streamer, use_graph, profile, sampling, procs, kv_start, out=None):
         """One run of the batch: prefill every micro-batch, then the decode loop.  ``procs``: the logits processors
         (``_logits_processors``) or None; on the first stage ``procs["history"]`` holds their starting history [B, S']
         (``input_ids`` plus any pad columns dropped before the run), which the first stage sends to the last one here,
-        once.  ``kv_start``: the per-row key starts of a left-padded batch, or None."""
+        once.  ``kv_start``: the per-row key starts of a left-padded batch, or None.  ``out``: ``_output_flags``; when
+        set, returns (result, scores, logits) (``_with_scores``)."""
         link, st, cfg = self.link, self.stage, self.cfg
         shape, sampling, procs = link.broadcast_object((tuple(input_ids.shape), sampling, procs) if link.first else None)
         prompt = None if procs is None else procs.pop("history")
         B, S = shape
+        if hasattr(st, "set_score_log"):             # off unless asked: the plain run keeps its launches
+            st.set_score_log(bool(out and out["scores"]), bool(out and out["logits"]), B, max_new)
         if hasattr(st, "set_sampling"):
             st.set_sampling(sampling)               # the last stage draws; greedy (None) restores the argmax path
             if sampling is not None and st.has_head:
@@ -811,7 +890,8 @@ class DistributedModel(torch.nn.Module):
                 if multi:
                     link.send_up(st.ids_dec[m][:b].clone(), 0)
         if ring is not None:
-            return self._decode_ring(ring, input_ids, B, S, b, n_mb, max_new, streamer, use_graph, profile, t0)
+            return self._with_scores(self._decode_ring(ring, input_ids, B, S, b, n_mb, max_new, streamer, use_graph, profile, t0),
+                                     S, out)
         # ---- decode rounds: micro-batches rotate through the stages; hidden [b,H] hops down, ids hop back up.
         # Sends are asynchronous; a slot's buffer is waited on only right before the next step overwrites it.
         sent_x = [None] * n_mb
@@ -893,4 +973,4 @@ class DistributedModel(torch.nn.Module):
         if streamer is not None and link.first:
             streamer.end()
         self.timers["generate_wall_s"] = time.perf_counter() - t0
-        return apply_eos(result, S, *self._eos)
+        return self._with_scores(apply_eos(result, S, *self._eos), S, out)

@@ -82,6 +82,10 @@ class CudaStage:
             self.pl_assistant: Optional["CudaStage"] = None
             # as an assistant (assist_draft): its 2-row catch-up input and hidden rows, allocated on first use
             self.asst: Optional[dict] = None
+            # generate's output_scores / output_logits (set_score_log): fp32 logs [columns, rows, V] of the scores and the
+            # raw logits, and per slot the log column {column, exit word} the picking kernel writes and advances
+            self.score_log: Optional[dict] = None
+            self.log_mode: Tuple[bool, bool] = (False, False)
 
     # ------------------------------------------------------------------------------------------ pieces
     def embed(self, ids: torch.Tensor) -> torch.Tensor:
@@ -143,6 +147,47 @@ class CudaStage:
             self.hist_log = torch.zeros(n_slots, self.max_batch, max(length, self.max_seq), dtype=torch.int32, device=dev)
             self.graphs.clear()                      # the captured kernels hold the old log's address
 
+    def set_score_log(self, scores: bool, logits: bool, rows: int = 0, n_cols: int = 0):
+        """Log every picked row's scores (HF's processed and warped values) and / or raw logits (fp32 of the bf16 logits)
+        into fp32 buffers [n_cols, rows, V]: the head of slot m writes its rows at m * (its batch) in the column its
+        counter names, and advances it.  Both False = off.  The buffers only grow; growing them or changing the mode
+        drops the captured decode graphs (they hold the buffer addresses and the launch's kernels).  Zeroes the columns."""
+        if not self.has_head:
+            return
+        mode = (bool(scores), bool(logits))
+        if mode != self.log_mode:
+            self.graphs.clear()
+        self.log_mode = mode
+        if not any(mode):
+            return
+        dev, V = self.device, self.cfg.vocab
+        lg = self.score_log
+        if lg is None:
+            lg = self.score_log = {"col": torch.zeros(len(self.slots), 2, dtype=torch.int32, device=dev),
+                                   "scores": None, "logits": None}
+        shape = (max(n_cols, 1), max(rows, 1))
+        for kind, on in zip(("scores", "logits"), mode):
+            t = lg[kind]
+            if on and (t is None or t.shape[0] < shape[0] or t.shape[1] < shape[1]):
+                old = (0, 0) if t is None else t.shape[:2]
+                lg[kind] = None                      # free the old buffer first
+                lg[kind] = torch.empty(max(shape[0], old[0]), max(shape[1], old[1]), V, dtype=torch.float32, device=dev)
+                self.graphs.clear()
+        lg["col"].zero_()
+
+    def _log(self, slot: int, B: int):
+        """slot's score log as the native picking calls take it, or None when off."""
+        if not any(self.log_mode):
+            return None
+        lg = self.score_log
+        return (lg["logits"] if self.log_mode[1] else None, lg["scores"] if self.log_mode[0] else None, lg["col"][slot],
+                slot * B)
+
+    def score_log_copy(self, kind: str, rows: int, n_cols: int) -> torch.Tensor:
+        """Columns 0..n_cols-1 of rows 0..rows-1 of the ``kind`` ("scores" / "logits") log: a new fp32 tensor
+        [n_cols, rows, V] (the next run does not change it)."""
+        return self.score_log[kind][:n_cols, :rows].clone()
+
     def fill_history(self, slot: int, prompt: torch.Tensor):
         """Row r of ``slot`` starts its token history with ``prompt[r]`` (int64 [b, S] on this device, pad columns included)."""
         nat.history_fill(prompt.contiguous(), self.hist_log[slot], self.hist_len[slot], self.hist_bits[slot], self.cfg.vocab)
@@ -151,17 +196,18 @@ class CudaStage:
         """next token for [B,H] rows -> ids_out [B] int64: greedy (bit-exact target: torch.argmax of bf16 logits) or, after
         ``set_sampling``, one draw per row from the warped distribution (csrc/sample.cu).  With logits processors on, both
         act on HF's processed scores and append the picked id to the row's history."""
+        log = self._log(slot, hidden.shape[0])
         if self.procs is not None:
-            self._head_processed(hidden, ids_out, slot)
+            self._head_processed(hidden, ids_out, slot, log)
             return
-        self._head_greedy(hidden, ids_out)
+        self._head_greedy(hidden, ids_out, log if self.sampling is None else None)
         if self.sampling is not None:
             B = hidden.shape[0]
             s = self.sampling
             nat.sample(self.logits_dec[:B], ids_out, self.sample_ctr[slot], self.sample_ws, s["temperature"], s["top_k"], s["top_p"],
-                       s["seed"] + 0x9E3779B97F4A7C15 * slot)
+                       s["seed"] + 0x9E3779B97F4A7C15 * slot, log=log)
 
-    def _head_processed(self, hidden: torch.Tensor, ids_out: torch.Tensor, slot: int):
+    def _head_processed(self, hidden: torch.Tensor, ids_out: torch.Tensor, slot: int, log=None):
         cfg, v = self.cfg, self.params.v
         B = hidden.shape[0]
         logits = self.logits_dec[:B]
@@ -173,22 +219,27 @@ class CudaStage:
             nat.gemm(self.hn[:B], v["head"], out=logits)
         hist = (self.hist_log[slot], self.hist_len[slot], self.hist_bits[slot], self.lp_params)
         if self.sampling is None:
-            nat.argmax_proc(logits, ids_out, *hist, self.lp_ws, self.lp_flags)
+            nat.argmax_proc(logits, ids_out, *hist, self.lp_ws, self.lp_flags, score_log=log)
         else:
             s = self.sampling
             nat.sample_proc(logits, ids_out, *hist, self.sample_ctr[slot], self.lp_ws, s["temperature"], s["top_k"], s["top_p"],
-                            s["seed"] + 0x9E3779B97F4A7C15 * slot, self.lp_flags)
+                            s["seed"] + 0x9E3779B97F4A7C15 * slot, self.lp_flags, score_log=log)
 
-    def _head_greedy(self, hidden: torch.Tensor, ids_out: torch.Tensor):
+    def _head_greedy(self, hidden: torch.Tensor, ids_out: torch.Tensor, log=None):
+        """``log``: a score log (``_log``): the argmax logs the logits it reads (tl_lmhead_argmax's two halves, the GEMV
+        and the argmax, run as separate calls then; the same launches)."""
         cfg, v = self.cfg, self.params.v
         B = hidden.shape[0]
-        if B <= gemv_max_rows():
+        if B <= gemv_max_rows() and log is None:
             nat.lmhead_argmax(hidden, v["head"], v["norm"], cfg.rms_eps, ids_out, self.logits_dec[:B], self.head_ws,
                               self.head_ctr)
+            return
+        if B <= gemv_max_rows():
+            nat.gemv(hidden, v["head"], out=self.logits_dec[:B], norm_w=v["norm"], eps=cfg.rms_eps, counter=self.head_ctr)
         else:
             nat.rmsnorm_fwd(hidden, v["norm"], cfg.rms_eps, out=self.hn[:B])
             nat.gemm(self.hn[:B], v["head"], out=self.logits_dec[:B])
-            nat.argmax_bf16(self.logits_dec[:B], ids_out, self.head_ws)
+        nat.argmax_bf16(self.logits_dec[:B], ids_out, self.head_ws, log=log)
 
     # ------------------------------------------------------------------------------------------ decode step
     def _decode_body_ring(self, slot: int, B: int, ring):
@@ -229,7 +280,7 @@ class CudaStage:
             self._decode_body(slot, B, ring)
             return
         ragged = self.slots[slot].ragged          # the captured launches differ (the _rows kernels, no decode chain)
-        key = (slot, B, ragged) if ring is None else (slot, B, ragged, id(ring))
+        key = (slot, B, ragged, self.log_mode if self.has_head else None) + (() if ring is None else (id(ring),))
         g = self.graphs.get(key)
         if g is None:
             # warm up outside capture (first-use attribute setting, tensor-map cache), restoring the state it touches
@@ -239,6 +290,7 @@ class CudaStage:
             hist_saved = None                                                   # ... nor join a row's token history
             if self.has_head and self.procs is not None:
                 hist_saved = (self.hist_len.clone(), self.hist_bits.clone())
+            col_saved = self.score_log["col"].clone() if self.has_head and any(self.log_mode) else None  # ... nor a column
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
@@ -250,6 +302,8 @@ class CudaStage:
                 self.sample_ctr.copy_(ctr_saved)
             if hist_saved is not None:
                 self.hist_len.copy_(hist_saved[0]); self.hist_bits.copy_(hist_saved[1])
+            if col_saved is not None:
+                self.score_log["col"].copy_(col_saved)
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):

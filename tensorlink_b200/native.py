@@ -22,6 +22,10 @@ class NativeError(RuntimeError):
     pass
 
 
+# the trailing arguments of the score-log (_log) entry points: raw log, score log, column counter, n_cols, B_total, row0,
+# stream
+_LOG_ARGS = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]
+
 _SIGS = {
     "tl_abi_version": (c_int, []),
     "tl_last_error": (c_char_p, []),
@@ -83,9 +87,12 @@ _SIGS = {
     "tl_lmhead_argmax": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_size_t,
                                  c_int, c_int, c_int, c_void_p, c_void_p]),
     "tl_argmax_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_void_p]),
+    "tl_argmax_bf16_log": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int] + _LOG_ARGS),
     "tl_sample_ws": (c_size_t, [c_int]),
     "tl_sample": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p, c_void_p, c_size_t,
                           c_void_p]),
+    "tl_sample_log": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p, c_void_p,
+                              c_size_t] + _LOG_ARGS),
     "tl_spec_accept_ws": (c_size_t, [c_int]),
     "tl_spec_accept": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_float,
                                ctypes.c_uint64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
@@ -94,6 +101,9 @@ _SIGS = {
     "tl_argmax_proc": (c_int, [c_void_p] * 6 + [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
     "tl_sample_proc": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p,
                                                 c_void_p, c_size_t, c_void_p]),
+    "tl_argmax_proc_log": (c_int, [c_void_p] * 6 + [c_int, c_void_p, c_size_t, c_int, c_int, c_int] + _LOG_ARGS),
+    "tl_sample_proc_log": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64,
+                                                    c_void_p, c_void_p, c_size_t] + _LOG_ARGS),
     "tl_advance_pos": (c_int, [c_void_p, c_void_p, c_int, c_void_p]),
     "tl_append_token": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "tl_swiglu_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
@@ -461,26 +471,56 @@ def lmhead_argmax(x, w, norm_w, eps, ids_out, logits_out, ws, counter: Optional[
            "tl_lmhead_argmax")
 
 
-def argmax_bf16(logits, ids_out, ws):
+def _log_args(log, M: int, V: int) -> list:
+    """The score log ``(raw, scores, col, row0)`` as the _log entry points take it: raw / scores fp32 [n_cols, B_total, V]
+    on the device (either may be None), col int32[2] {column, exit word}, launch row m logged at row row0 + m."""
+    raw, scores, col, row0 = log
+    ref = raw if raw is not None else scores
+    if ref is None:
+        raise NativeError("score log: neither a raw nor a score buffer")
+    for t in (raw, scores):
+        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous() or t.dim() != 3
+                              or t.shape != ref.shape or t.shape[2] != V):
+            raise NativeError(f"score log buffers must be contiguous fp32 CUDA tensors [n_cols, B_total, {V}] of one shape")
+    if col is None:
+        raise NativeError("score log: no column counter")
+    _i32(col)
+    if col.numel() < 2:
+        raise NativeError("score log: the column counter is int32[2] {column, exit word}")
+    return [_p(raw), _p(scores), _p(col), ref.shape[0], ref.shape[1], int(row0), _stream()]
+
+
+def argmax_bf16(logits, ids_out, ws, log=None):
+    """``log``: None, or a score log (``_log_args``) that receives the logits as raw values and as scores."""
     require_device()
     _bf16(logits)
     M, V = logits.shape
-    _check(load().tl_argmax_bf16(_p(logits), _p(ids_out), _p(ws), ws.numel() * ws.element_size(), M, V, _stream()),
-           "tl_argmax_bf16")
+    if log is None:
+        _check(load().tl_argmax_bf16(_p(logits), _p(ids_out), _p(ws), ws.numel() * ws.element_size(), M, V, _stream()),
+               "tl_argmax_bf16")
+        return
+    _check(load().tl_argmax_bf16_log(_p(logits), _p(ids_out), _p(ws), ws.numel() * ws.element_size(), M, V,
+                                     *_log_args(log, M, V)), "tl_argmax_bf16_log")
 
 
 def sample_ws(M: int) -> int:
     return int(load().tl_sample_ws(M))
 
 
-def sample(logits, ids_out, counters, ws, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0):
-    """ids_out[m] ~ softmax(top-p(top-k(logits[m] / temperature))); ``counters`` int32[M] advance by one per call."""
+def sample(logits, ids_out, counters, ws, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
+           log=None):
+    """ids_out[m] ~ softmax(top-p(top-k(logits[m] / temperature))); ``counters`` int32[M] advance by one per call.
+    ``log``: None, or a score log (``_log_args``): raw logits, and logits / temperature on the kept set, -inf elsewhere."""
     require_device()
     _bf16(logits)
     M, V = logits.shape
     assert ids_out.dtype == torch.int64 and counters.dtype == torch.int32 and counters.numel() >= M
-    _check(load().tl_sample(_p(logits), _p(ids_out), M, V, float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1),
-                            _p(counters), _p(ws), ws.numel() * ws.element_size(), _stream()), "tl_sample")
+    args = [_p(logits), _p(ids_out), M, V, float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1),
+            _p(counters), _p(ws), ws.numel() * ws.element_size()]
+    if log is None:
+        _check(load().tl_sample(*args, _stream()), "tl_sample")
+    else:
+        _check(load().tl_sample_log(*args, *_log_args(log, M, V)), "tl_sample_log")
 
 
 def spec_accept_ws(K: int) -> int:
@@ -533,29 +573,38 @@ def history_fill(prompt, log, length, bits, V: int):
     _check(load().tl_history_fill(_p(prompt), _p(log), _p(length), _p(bits), M, S, L, V, _stream()), "tl_history_fill")
 
 
-def argmax_proc(logits, ids_out, log, length, bits, params, ws, flags: int = 0):
-    """ids_out[m] = torch.argmax of HF's processed fp32 scores of logits[m]; appends the id to row m's history."""
+def argmax_proc(logits, ids_out, log, length, bits, params, ws, flags: int = 0, score_log=None):
+    """ids_out[m] = torch.argmax of HF's processed fp32 scores of logits[m]; appends the id to row m's history.
+    ``score_log``: None, or a score log (``_log_args``): raw logits and the processed scores."""
     require_device()
     _bf16(logits)
     M, V = logits.shape
     L = _history(log, length, bits, M, V)
     assert ids_out.dtype == torch.int64 and params.dtype == torch.int32 and params.numel() >= LP_PARAMS
-    _check(load().tl_argmax_proc(_p(logits), _p(ids_out), _p(log), _p(length), _p(bits), _p(params), flags, _p(ws),
-                                 ws.numel() * ws.element_size(), M, V, L, _stream()), "tl_argmax_proc")
+    args = [_p(logits), _p(ids_out), _p(log), _p(length), _p(bits), _p(params), flags, _p(ws), ws.numel() * ws.element_size(),
+            M, V, L]
+    if score_log is None:
+        _check(load().tl_argmax_proc(*args, _stream()), "tl_argmax_proc")
+    else:
+        _check(load().tl_argmax_proc_log(*args, *_log_args(score_log, M, V)), "tl_argmax_proc_log")
 
 
 def sample_proc(logits, ids_out, log, length, bits, params, counters, ws, temperature: float = 1.0, top_k: int = 0,
-                top_p: float = 1.0, seed: int = 0, flags: int = 0):
-    """``sample`` over HF's processed fp32 scores; appends the drawn id to row m's history."""
+                top_p: float = 1.0, seed: int = 0, flags: int = 0, score_log=None):
+    """``sample`` over HF's processed fp32 scores; appends the drawn id to row m's history.  ``score_log``: None, or a
+    score log (``_log_args``): raw logits, and processed / temperature on the kept set, -inf elsewhere."""
     require_device()
     _bf16(logits)
     M, V = logits.shape
     L = _history(log, length, bits, M, V)
     assert ids_out.dtype == torch.int64 and counters.dtype == torch.int32 and counters.numel() >= M
     assert params.dtype == torch.int32 and params.numel() >= LP_PARAMS
-    _check(load().tl_sample_proc(_p(logits), _p(ids_out), _p(log), _p(length), _p(bits), _p(params), flags, M, V, L,
-                                 float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1), _p(counters),
-                                 _p(ws), ws.numel() * ws.element_size(), _stream()), "tl_sample_proc")
+    args = [_p(logits), _p(ids_out), _p(log), _p(length), _p(bits), _p(params), flags, M, V, L, float(temperature),
+            int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1), _p(counters), _p(ws), ws.numel() * ws.element_size()]
+    if score_log is None:
+        _check(load().tl_sample_proc(*args, _stream()), "tl_sample_proc")
+    else:
+        _check(load().tl_sample_proc_log(*args, *_log_args(score_log, M, V)), "tl_sample_proc_log")
 
 
 def lp_params(penalty: float, ngram: int, min_new: int, prompt_len: int, eos_ids) -> torch.Tensor:
