@@ -17,7 +17,7 @@ import numbers
 import os
 
 import time
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 from typing import Any, Callable, Dict, Optional, Union
 
 import torch
@@ -75,6 +75,22 @@ def _check_unconsumed(kwargs: dict, what: str):
                                       "(it would be silently ignored otherwise)")
 
 
+# What a generate call may need of its stage, each with the attribute that provides it.  The CUDA stage provides all
+# of them; another stage (the CPU stages of the tests) provides those whose attribute it has.
+_STAGE_FEATURES = {"scores": "set_score_log", "sampling": "set_sampling", "processors": "set_logits_processors",
+                   "drafts": "prompt_lookup_begin", "kv_start": "supports_kv_start", "check": "check"}
+
+
+def _stage_supports(stage, feature: str, what: Optional[str] = None) -> bool:
+    """Whether ``stage`` provides ``feature`` (a key of _STAGE_FEATURES).  With ``what``, a stage without it raises
+    NotImplementedError("<what> needs the CUDA stage")."""
+    from .stage import CudaStage
+    ok = isinstance(stage, CudaStage) or bool(getattr(stage, _STAGE_FEATURES[feature], False))
+    if not ok and what is not None:
+        raise NotImplementedError(f"{what} needs the CUDA stage")
+    return ok
+
+
 def _logits_processors(repetition_penalty=None, no_repeat_ngram_size=None, min_new_tokens=None,
                        eos_token_id=None) -> Optional[dict]:
     """HF's ``repetition_penalty`` / ``no_repeat_ngram_size`` / ``min_new_tokens`` as {penalty, ngram, min_new, eos}, or
@@ -124,10 +140,7 @@ def _prompt_lookup(num_tokens, ngram, shape, max_new, max_seq, sampling=None, pr
         raise NotImplementedError("prompt_lookup_num_tokens on a pipeline of more than one stage")
     if len(_eos_list(eos_token_id)) > PL_MAX_EOS:
         raise NotImplementedError(f"prompt_lookup_num_tokens with more than {PL_MAX_EOS} EOS ids")
-    from .stage import CudaStage
-    if not isinstance(stage, CudaStage):
-        raise NotImplementedError(f"prompt_lookup_num_tokens{' with do_sample=True' if sampling is not None else ''} needs "
-                                  "the CUDA stage")
+    _stage_supports(stage, "drafts", f"prompt_lookup_num_tokens{' with do_sample=True' if sampling is not None else ''}")
     return {"K": K, "ngram": int(n)}
 
 
@@ -171,10 +184,8 @@ def _assisted(target, assistant, num_tokens, shape, max_new, sampling=None, proc
         raise NotImplementedError("assistant_model with repetition_penalty / no_repeat_ngram_size / min_new_tokens")
     if target.world > 1 or assistant.world > 1:
         raise NotImplementedError("assistant_model with a model or an assistant on a pipeline of more than one stage")
-    from .stage import CudaStage
-    if not isinstance(target.stage, CudaStage) or not isinstance(assistant.stage, CudaStage):
-        raise NotImplementedError(f"assistant_model{' with do_sample=True' if sampling is not None else ''} needs the CUDA "
-                                  "stage on the model and on the assistant")
+    for st in (target.stage, assistant.stage):
+        _stage_supports(st, "drafts", f"assistant_model{' with do_sample=True' if sampling is not None else ''}")
     if _device_key(assistant.stage.device) != _device_key(target.stage.device):
         raise NotImplementedError(f"assistant_model on {assistant.stage.device} for a model on {target.stage.device} "
                                   "(both run on one device)")
@@ -266,6 +277,29 @@ def _eos_list(eos_token_id):
     if isinstance(eos_token_id, torch.Tensor):              # HF accepts an int, a list or a tensor of ids
         return [int(e) for e in eos_token_id.reshape(-1).tolist()]
     return [int(e) for e in eos_token_id] if isinstance(eos_token_id, (list, tuple)) else [int(eos_token_id)]
+
+
+@dataclass(frozen=True)
+class _Request:
+    """One ``generate`` call, parsed once (``DistributedModel._request``) and the same on every rank."""
+    max_new: int
+    shape: tuple                      # [rows, S] of the prompt the run sees (from the first rank, as those below)
+    sampling: Optional[dict] = None   # {temperature, top_k, top_p, seed}, or None: greedy
+    eos: tuple = ()                   # the EOS ids
+    pad_token_id: Optional[int] = None
+    procs: Optional[dict] = None      # _logits_processors
+    draft: Optional[dict] = None      # the draft source: _prompt_lookup or _assisted, or None
+    out: Optional[dict] = None        # _output_flags
+    streamer: Any = None
+    use_graph: bool = True
+    profile: bool = False
+    # a left-padded batch either as the leading columns that are pad in every row (dropped before the run, back in the
+    # result) and the per-row key starts of the rest, or, on a stage without per-row key starts, as {real length:
+    # [rows]}; and the logits processors' starting history
+    pad_cols: Optional[torch.Tensor] = None
+    kv_start: Optional[list] = None
+    groups: Optional[dict] = None
+    history: Optional[torch.Tensor] = None
 
 
 def _all_rows_finished(tokens: torch.Tensor, eos_ids) -> bool:
@@ -500,11 +534,9 @@ class DistributedModel(torch.nn.Module):
 
     # ------------------------------------------------------------------------------------------ peer-memory decode
     def _peer_ring(self, n_mb: int):
-        """The mailbox ring for decode hops (p2p/peer.py), or None: TL_P2P=nccl, or a stage that is not the CUDA one
+        """The mailbox ring for decode hops (p2p/peer.py), or None: TL_P2P=nccl, or stages that are not on CUDA devices
         (the gloo tests drive this class with a CPU stage).  Built collectively on first use."""
-        import os
-        from .stage import CudaStage
-        if os.environ.get("TL_P2P", "peer") == "nccl" or not isinstance(self.stage, CudaStage):
+        if os.environ.get("TL_P2P", "peer") == "nccl" or self.device.type != "cuda":
             return None
         if getattr(self, "_ring", None) is None:
             from ..p2p.peer import PeerRing
@@ -512,20 +544,21 @@ class DistributedModel(torch.nn.Module):
             self._ring = PeerRing(self.link, len(st.slots), st.max_batch, self.cfg.hidden, st.max_seq, self.device)
         return self._ring
 
-    def _decode_ring(self, ring, input_ids, B, S, b, n_mb, max_new, streamer, use_graph, profile, t0):
+    def _decode_ring(self, ring, input_ids, req: _Request, b, n_mb, t0):
         """Decode rounds with every hop on peer memory.  The host only enqueues: max_new-1 graph replays per
         micro-batch (wait -> layers -> store into the neighbour -> signal), no synchronisation until the end; the
         first stage logs each token column on the device (``ring.out_log``)."""
         link, st, dev = self.link, self.stage, self.device
+        streamer, max_new = req.streamer, req.max_new
+        B = req.shape[0]
         span = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
         span[0].record()
         step_done = []
-        eos_ids = _eos_list(self._eos[0])
         n_cols = max_new                              # token columns that will exist when the loop ends
         for step in range(max_new):
             for m in range(n_mb):
                 if step < max_new - 1:
-                    st.decode(m, b, use_graph, ring=ring)
+                    st.decode(m, b, req.use_graph, ring=ring)
                 elif link.first:                                   # last column: nothing left to compute
                     ring.wait_ids(m)
                     ring.log_token(m, b)
@@ -533,12 +566,12 @@ class DistributedModel(torch.nn.Module):
                 ev = torch.cuda.Event()
                 ev.record()
                 step_done.append(ev)
-            if eos_ids and step < max_new - 1 and (step + 1) % EOS_CHECK_EVERY == 0:
+            if req.eos and step < max_new - 1 and (step + 1) % EOS_CHECK_EVERY == 0:
                 # HF stops once every row has emitted EOS.  Columns 0..step are logged on the first stage; all ranks
                 # drain their queues (no persistent kernel is in flight during the collective) and agree on stopping.
                 torch.cuda.synchronize(dev)
                 flag = torch.zeros(1, dtype=torch.int32, device=dev)
-                if link.first and _all_rows_finished(ring.out_log[:n_mb, :b, :step + 1].reshape(B, step + 1), eos_ids):
+                if link.first and _all_rows_finished(ring.out_log[:n_mb, :b, :step + 1].reshape(B, step + 1), req.eos):
                     flag.fill_(1)
                 link.broadcast(flag, 0)
                 if int(flag.item()):
@@ -551,66 +584,49 @@ class DistributedModel(torch.nn.Module):
                 streamer.put(ring.out_log[:n_mb, :b, step].reshape(-1).cpu())
         torch.cuda.synchronize(dev)
         ring.check()
-        if hasattr(st, "check"):
-            st.check()
-        if profile:
+        if req.profile:
             self.timers["decode_span_s"] = span[0].elapsed_time(span[1]) * 1e-3
             self.timers["decode_busy_s"] = self.timers["decode_span_s"] - float(ring.wait_ns.item()) * 1e-9
-        if link.first:
-            out_tokens = ring.out_log[:n_mb, :b, :n_cols].reshape(B, n_cols)
-            result = torch.cat([input_ids.to(dev), out_tokens], dim=1)
-        else:
-            result = torch.empty(B, S + n_cols, dtype=torch.int64, device=dev)
-        link.broadcast(result, 0)
-        if streamer is not None and link.first:
-            streamer.end()
-        self.timers["generate_wall_s"] = time.perf_counter() - t0
-        return apply_eos(result, S, *self._eos)
+        tokens = ring.out_log[:n_mb, :b, :n_cols].reshape(B, n_cols) if link.first else None
+        return self._finish(req, input_ids, tokens, n_cols, t0)
 
-    def _generate_left_padded(self, input_ids, groups, shape, max_new, streamer, use_graph, sampling):
+    def _generate_left_padded(self, input_ids, req: _Request):
         """HF semantics for a left-padded batch on a stage without per-row key starts (``supports_kv_start``): every row
         attends to its own tokens only, at positions 0..L-1.  Rows of equal real length are generated together (one
         uniform run per length: the KV cache and RoPE positions of a run start at the row's first real token, so no pad
-        key exists to be masked); the result keeps HF's layout [pads | prompt | new tokens | pad_token_id...]."""
-        if streamer is not None:
-            raise NotImplementedError("streamer with a padded batch (rows finish in separate runs)")
-        eos, pad = self._eos
-        pad_id = pad if pad is not None else (_eos_list(eos)[0] if eos is not None else 0)
-        first = self.link.first
-        B, S = shape
-        out = torch.full((B, S + max_new), int(pad_id), dtype=torch.int64, device=self.device)
+        key exists to be masked); the result keeps HF's layout [pads | prompt | new tokens | pad_token_id...].  Sampled,
+        the run of length L draws with the seed + L."""
+        dev, first = self.device, self.link.first
+        B, S = req.shape
+        pad_id = req.pad_token_id if req.pad_token_id is not None else (req.eos[0] if req.eos else 0)
+        out = torch.full((B, S + req.max_new), pad_id, dtype=torch.int64, device=dev)
         if first:
-            out[:, :S] = input_ids.to(self.device)
+            out[:, :S] = input_ids.to(dev)
         longest = 0
-        for L in sorted(groups):
-            rows = groups[L]
+        for L in sorted(req.groups):
+            rows = req.groups[L]
             sub = input_ids[rows][:, S - L:].contiguous() if first else None
-            kw = dict(max_new_tokens=max_new, use_graph=use_graph, eos_token_id=eos, pad_token_id=pad)
-            if sampling is not None:
-                kw.update(do_sample=True, temperature=sampling["temperature"], top_k=sampling["top_k"], top_p=sampling["top_p"],
-                          seed=sampling["seed"] + L)
-            got = self.generate(sub, **kw)
+            sampling = None if req.sampling is None else dict(req.sampling, seed=req.sampling["seed"] + L)
+            got = self._generate_batch(sub, replace(req, shape=(len(rows), L), groups=None, sampling=sampling))
             n_new = got.shape[1] - L
-            out[torch.as_tensor(rows, device=self.device), S:S + n_new] = got[:, L:].to(self.device)
+            out[torch.as_tensor(rows, device=dev), S:S + n_new] = got[:, L:].to(dev)
             longest = max(longest, n_new)
-        self._eos = (eos, pad)
         out = out[:, :S + longest].contiguous()
-        if self.world > 1:
-            self.link.broadcast(out, 0)              # every rank returns the whole result, prompt and pads included
+        self.link.broadcast(out, 0)                  # every rank returns the whole result, prompt and pads included
         return out
 
-    def _generate_lookup(self, input_ids, max_new, streamer, use_graph, lookup, sampling):
+    def _generate_lookup(self, input_ids, req: _Request):
         """Generation of one row with prompt-lookup drafts (``_prompt_lookup``) or an assistant's (``_assisted``) on the
-        one CUDA stage, greedy or sampled (``sampling``): prefill, the first token from the head, then verify steps
+        one CUDA stage, greedy or sampled (``req.sampling``): prefill, the first token from the head, then verify steps
         (ml/stage.py ``prompt_lookup_step``), each drafting K tokens on the device (from the row's history, or by the assistant,
         whose cache starts with the prompt's prefill) and emitting 1..K+1 tokens.  The host replays rounds of
         r = max(1, (max_new - count) // (K+1)) steps (at most EOS_CHECK_EVERY with ``eos_token_id``), so no step runs
         once max_new tokens are out, and reads the token count once per round."""
-        st, dev = self.stage, self.device
-        K, asst = lookup["K"], lookup.get("assistant")
+        st, dev, max_new, streamer = self.stage, self.device, req.max_new, req.streamer
+        K, asst = req.draft["K"], req.draft.get("assistant")
         S = input_ids.shape[1]
-        st.set_sampling(sampling)                  # no logits processors: the plain argmax or sampling head
-        if sampling is not None:
+        st.set_sampling(req.sampling)              # no logits processors: the plain argmax or sampling head
+        if req.sampling is not None:
             st.sample_ctr.zero_()                  # a seed names ONE set of streams (ml/stage.py STREAM_PL_ROWS)
         st.set_logits_processors(None)
         t0 = time.perf_counter()
@@ -618,14 +634,13 @@ class DistributedModel(torch.nn.Module):
         x = st.prefill(st.embed(ids), 0, 0)
         first = st.ids_dec[0][:1]
         st.head_argmax(x[:, -1, :].contiguous(), first, 0)
-        eos_ids = _eos_list(self._eos[0])
         steps, count = 0, 0
         tokens = torch.zeros(0, dtype=torch.int64)
         if max_new >= 1:
             if asst is not None:
                 asst.prefill(asst.embed(ids), 0, 0)
-            st.prompt_lookup_begin(torch.cat([ids, first.view(1, 1)], dim=1), K, lookup["ngram"], S + max_new, eos_ids,
-                                   assistant=asst)
+            st.prompt_lookup_begin(torch.cat([ids, first.view(1, 1)], dim=1), K, req.draft["ngram"], S + max_new,
+                                   list(req.eos), assistant=asst)
             while True:
                 count = st.prompt_lookup_count()
                 new = st.prompt_lookup_tokens(tokens.numel(), count)
@@ -633,20 +648,47 @@ class DistributedModel(torch.nn.Module):
                 if streamer is not None:
                     for j in range(new.numel()):
                         streamer.put(new[j:j + 1])
-                if count >= max_new or any(int(t) in eos_ids for t in new):
+                if count >= max_new or any(int(t) in req.eos for t in new):
                     break
                 r = max(1, (max_new - count) // (K + 1))
-                if eos_ids:
+                if req.eos:
                     r = min(r, EOS_CHECK_EVERY)
                 for _ in range(r):
-                    st.prompt_lookup_step(use_graph)
+                    st.prompt_lookup_step(req.use_graph)
                 steps += r
         self.timers["prompt_lookup_steps" if asst is None else "assisted_steps"] = steps
-        result = torch.cat([ids, tokens[:max_new].to(dev).view(1, -1)], dim=1)
-        if streamer is not None:
-            streamer.end()
+        tokens = tokens[:max_new].view(1, -1)
+        return self._finish(req, ids, tokens, tokens.shape[1], t0)
+
+    def _finish(self, req: _Request, input_ids, tokens, n_cols: int, t0: float):
+        """The end of every run: the result [B, S + n_cols], the prompt then the first ``n_cols`` columns of the first
+        stage's ``tokens``, on every rank; the stage's error check; HF's EOS cut (``apply_eos``); the streamer's end;
+        ``timers["generate_wall_s"]``.  With ``req.out``, returns (result, logs): the last stage's score logs of the
+        generated columns the cut kept, on every rank, as {"scores" / "logits": a tuple of fp32 [B, V] tensors}."""
+        link, dev = self.link, self.device
+        B, S = req.shape
+        if link.first:
+            result = torch.cat([input_ids.to(dev), tokens[:, :n_cols].to(dev)], dim=1)
+        else:
+            result = torch.empty(B, S + n_cols, dtype=torch.int64, device=dev)
+        link.broadcast(result, 0)
+        if _stage_supports(self.stage, "check"):
+            self.stage.check()
+        if req.streamer is not None and link.first:
+            req.streamer.end()
         self.timers["generate_wall_s"] = time.perf_counter() - t0
-        return apply_eos(result, S, *self._eos)
+        result = apply_eos(result, S, list(req.eos) or None, req.pad_token_id)
+        logs, n_new = {}, result.shape[1] - S
+        for kind in ("scores", "logits"):
+            if req.out is None or not req.out[kind]:
+                continue
+            if link.last:
+                t = self.stage.score_log_copy(kind, B, n_new)
+            else:
+                t = torch.empty(n_new, B, self.cfg.vocab, dtype=torch.float32, device=dev)
+            link.broadcast(t, self.world - 1)
+            logs[kind] = tuple(t.unbind(0))
+        return result if req.out is None else (result, logs)
 
     # ------------------------------------------------------------------------------------------ generate
     @torch.no_grad()
@@ -709,6 +751,26 @@ class DistributedModel(torch.nn.Module):
         without ``supports_kv_start``, or on a non-CUDA stage, ``return_dict_in_generate=True`` raises
         NotImplementedError.  ``compute_transition_scores`` turns ``scores`` into per-token log-probabilities."""
         input_ids = kwargs.pop("input_ids", args[0] if args else None)
+        req, input_ids = self._request(input_ids, kwargs)
+        if req.groups is not None:
+            return self._generate_left_padded(input_ids, req)
+        result = (self._generate_lookup if req.draft is not None else self._generate_batch)(input_ids, req)
+        if req.out is not None:
+            result, logs = result
+        if req.pad_cols is not None and req.pad_cols.shape[1]:       # the dropped pad columns return in the result
+            result = torch.cat([req.pad_cols.to(result.device), result], dim=1)
+        if req.out is None:
+            return result
+        from transformers.generation import GenerateDecoderOnlyOutput
+        return GenerateDecoderOnlyOutput(sequences=result, **logs)
+
+    def _request(self, input_ids, kwargs: dict):
+        """``generate``'s keywords as one _Request, and ``input_ids`` as the run sees it (without the columns that are pad
+        in every row).  Every rank parses its own keywords and checks every combination of modes, and of a mode and its
+        stage, before any stage work; then one broadcast hands every rank what only the first one knows: the prompt's
+        shape and padding, the logits processors' starting history and the sampling seed (``torch.initial_seed()``
+        unless given)."""
+        link, st = self.link, self.stage
         max_new = int(kwargs.pop("max_new_tokens", 20))
         streamer = kwargs.pop("streamer", None)
         use_graph = kwargs.pop("use_graph", True)
@@ -721,9 +783,9 @@ class DistributedModel(torch.nn.Module):
                         "top_p": 1.0 if top_p is None else float(top_p), "seed": int(torch.initial_seed() if seed is None else seed)}
             if sampling["temperature"] <= 0 or not (0 < sampling["top_p"] <= 1) or sampling["top_k"] < 0:
                 raise ValueError(f"invalid sampling parameters {sampling}")
-        self._eos = (kwargs.pop("eos_token_id", None), kwargs.pop("pad_token_id", None))
+        eos_token_id, pad_token_id = kwargs.pop("eos_token_id", None), kwargs.pop("pad_token_id", None)
         procs = _logits_processors(kwargs.pop("repetition_penalty", None), kwargs.pop("no_repeat_ngram_size", None),
-                                   kwargs.pop("min_new_tokens", None), self._eos[0])
+                                   kwargs.pop("min_new_tokens", None), eos_token_id)
         mask = kwargs.pop("attention_mask", None)
         lookup = kwargs.pop("prompt_lookup_num_tokens", None)
         ngram = kwargs.pop("max_matching_ngram_size", None) if lookup is not None else None
@@ -737,56 +799,48 @@ class DistributedModel(torch.nn.Module):
             raise NotImplementedError("assistant_model together with prompt_lookup_num_tokens: pick one draft source")
         if out is not None and (lookup is not None or assistant is not None):
             raise NotImplementedError("return_dict_in_generate=True with prompt_lookup_num_tokens / assistant_model")
-        link, st, cfg = self.link, self.stage, self.cfg
-        if out is not None and not hasattr(st, "set_score_log"):
-            raise NotImplementedError("return_dict_in_generate=True needs the CUDA stage")
-        groups, padded = None, None
+        if out is not None:
+            _stage_supports(st, "scores", "return_dict_in_generate=True")
+        pad_cols = kv_start = groups = None
         if link.first and mask is not None:
             if tuple(mask.shape) != tuple(input_ids.shape):
                 raise ValueError(f"attention_mask shape {tuple(mask.shape)} != input_ids shape {tuple(input_ids.shape)}")
-            if getattr(st, "supports_kv_start", False):
+            if _stage_supports(st, "kv_start"):
                 p = _left_pad_starts(mask)
-                # (pad columns common to every row, per-row key starts); the dropped columns return in the result
-                padded = None if p is None else (input_ids[:, :p[0]].cpu(), p[1])
-                if padded is not None:
+                if p is not None:
+                    pad_cols, kv_start = input_ids[:, :p[0]].cpu(), p[1]
                     input_ids = input_ids[:, p[0]:]
             else:
-                g = _left_pad_groups(mask)
-                groups = None if g is None else (g, tuple(input_ids.shape))
+                groups = _left_pad_groups(mask)
+        shape = tuple(input_ids.shape) if input_ids is not None else (1, 0)
+        draft = None
         if assistant is not None:
-            lookup = _assisted(self, assistant, n_assist, tuple(input_ids.shape), max_new, sampling, procs)
+            draft = _assisted(self, assistant, n_assist, shape, max_new, sampling, procs)
         elif lookup is not None:
-            lookup = _prompt_lookup(lookup, ngram, tuple(input_ids.shape) if input_ids is not None else (1, 0), max_new,
-                                    self.max_seq, sampling, procs, self.world, st, self._eos[0])
-        if lookup is not None:
-            result = self._generate_lookup(input_ids, max_new, streamer, use_graph, lookup, sampling)
-            if padded is not None and padded[0].shape[1]:
-                result = torch.cat([padded[0].to(result.device), result], dim=1)
-            return result
+            draft = _prompt_lookup(lookup, ngram, shape, max_new, self.max_seq, sampling, procs, self.world, st, eos_token_id)
+        else:
+            if sampling is not None:
+                _stage_supports(st, "sampling", "do_sample=True")
+            if procs is not None:
+                _stage_supports(st, "processors", "repetition_penalty / no_repeat_ngram_size / min_new_tokens")
+        history = None
+        if procs is not None and link.first:         # the starting history: every column, the dropped pad columns too
+            history = input_ids.cpu() if pad_cols is None else torch.cat([pad_cols, input_ids.cpu()], dim=1)
         if self.world > 1:
-            groups, padded, procs = link.broadcast_object((groups, padded, procs))
-        if procs is not None and not hasattr(st, "set_logits_processors"):
-            raise NotImplementedError("repetition_penalty / no_repeat_ngram_size / min_new_tokens need the CUDA stage")
-        if groups is not None:
-            if procs is not None:                # the grouped runs would see each row's history without its pads
+            shape, pad_cols, kv_start, groups, history, sampling = link.broadcast_object(
+                (shape, pad_cols, kv_start, groups, history, sampling) if link.first else None)
+        if groups is not None:                       # the grouped runs generate each real length in a run of its own:
+            if procs is not None:                    # each row's history would lack its pads
                 raise NotImplementedError("repetition_penalty / no_repeat_ngram_size / min_new_tokens with a left-padded "
                                           "batch need a stage with per-row key starts (supports_kv_start)")
-            if out is not None:                  # the grouped runs return their rows in separate calls
+            if out is not None:                      # the rows come back in separate runs
                 raise NotImplementedError("return_dict_in_generate=True with a left-padded batch needs a stage with "
                                           "per-row key starts (supports_kv_start)")
-            return self._generate_left_padded(input_ids, groups[0], groups[1], max_new, streamer, use_graph, sampling)
-        if procs is not None and link.first:     # the starting history: every column, the dropped pad columns too
-            procs["history"] = input_ids.cpu() if padded is None else torch.cat([padded[0], input_ids.cpu()], dim=1)
-        result = self._generate_batch(input_ids, max_new, streamer, use_graph, profile, sampling, procs,
-                                      None if padded is None else padded[1], **({} if out is None else {"out": out}))
-        if out is not None:
-            result, scores, logits = result
-        if padded is not None and padded[0].shape[1]:
-            result = torch.cat([padded[0].to(result.device), result], dim=1)
-        if out is None:
-            return result
-        from transformers.generation import GenerateDecoderOnlyOutput
-        return GenerateDecoderOnlyOutput(sequences=result, scores=scores, logits=logits)
+            if streamer is not None:                 # the rows finish in separate runs
+                raise NotImplementedError("streamer with a padded batch (rows finish in separate runs)")
+        pad_token_id = None if pad_token_id is None else int(pad_token_id)
+        return _Request(max_new, shape, sampling, tuple(_eos_list(eos_token_id)), pad_token_id, procs, draft, out, streamer,
+                        use_graph, profile, pad_cols, kv_start, groups, history), input_ids
 
     def compute_transition_scores(self, sequences: torch.Tensor, scores, normalize_logits: bool = False) -> torch.Tensor:
         """HF ``compute_transition_scores`` without beams: [B, len(scores)] = each emitted token's score at its column,
@@ -801,50 +855,22 @@ class DistributedModel(torch.nn.Module):
         rows = torch.arange(scores[0].shape[0], device=sequences.device).view(-1, 1) * V
         return stacked.gather(0, sequences[:, sequences.shape[-1] - T:] + rows)
 
-    def _with_scores(self, result: torch.Tensor, S: int, out):
-        """``result`` of a finished run, or with ``out`` (``_output_flags``) (result, scores, logits): the last stage's
-        score log, columns 0..n_new-1 for the n_new generated columns ``result`` kept, on every rank; scores and logits
-        are each a tuple of n_new fp32 [B, V] tensors, or None when not asked for."""
-        if out is None:
-            return result
-        link, st = self.link, self.stage
-        B, n_new = result.shape[0], result.shape[1] - S
-        got = []
-        for kind in ("scores", "logits"):
-            if not out[kind]:
-                got.append(None)
-                continue
-            if link.last:
-                t = st.score_log_copy(kind, B, n_new)
-            else:
-                t = torch.empty(n_new, B, self.cfg.vocab, dtype=torch.float32, device=self.device)
-            link.broadcast(t, self.world - 1)
-            got.append(tuple(t.unbind(0)))
-        return (result, *got)
-
-    def _generate_batch(self, input_ids, max_new, streamer, use_graph, profile, sampling, procs, kv_start, out=None):
-        """One run of the batch: prefill every micro-batch, then the decode loop.  ``procs``: the logits processors
-        (``_logits_processors``) or None; on the first stage ``procs["history"]`` holds their starting history [B, S']
-        (``input_ids`` plus any pad columns dropped before the run), which the first stage sends to the last one here,
-        once.  ``kv_start``: the per-row key starts of a left-padded batch, or None.  ``out``: ``_output_flags``; when
-        set, returns (result, scores, logits) (``_with_scores``)."""
+    def _generate_batch(self, input_ids, req: _Request):
+        """One run of the batch: prefill every micro-batch, then the decode loop.  With logits processors, the last
+        stage starts every row's history with ``req.history`` [B, S'] (``input_ids`` plus any pad columns dropped
+        before the run).  Returns as ``_finish``."""
         link, st, cfg = self.link, self.stage, self.cfg
-        shape, sampling, procs = link.broadcast_object((tuple(input_ids.shape), sampling, procs) if link.first else None)
-        prompt = None if procs is None else procs.pop("history")
-        B, S = shape
-        if hasattr(st, "set_score_log"):             # off unless asked: the plain run keeps its launches
+        B, S = req.shape
+        max_new, streamer, procs, out = req.max_new, req.streamer, req.procs, req.out
+        if _stage_supports(st, "scores"):            # off unless asked: the plain run keeps its launches
             st.set_score_log(bool(out and out["scores"]), bool(out and out["logits"]), B, max_new)
-        if hasattr(st, "set_sampling"):
-            st.set_sampling(sampling)               # the last stage draws; greedy (None) restores the argmax path
-            if sampling is not None and st.has_head:
+        if _stage_supports(st, "sampling"):
+            st.set_sampling(req.sampling)           # the last stage draws; greedy (None) restores the argmax path
+            if req.sampling is not None and st.has_head:
                 st.sample_ctr.zero_()               # a seed names ONE stream: the same call reproduces its tokens
-        elif sampling is not None:
-            raise NotImplementedError("sampling needs the CUDA stage")
-        if hasattr(st, "set_logits_processors"):
-            st.set_logits_processors(None if procs is None else dict(procs, prompt_len=prompt.shape[1]),
-                                     0 if procs is None else prompt.shape[1] + max_new)
-        elif procs is not None:
-            raise NotImplementedError("repetition_penalty / no_repeat_ngram_size / min_new_tokens need the CUDA stage")
+        if _stage_supports(st, "processors"):
+            st.set_logits_processors(None if procs is None else dict(procs, prompt_len=req.history.shape[1]),
+                                     0 if procs is None else req.history.shape[1] + max_new)
         n_mb = min(self.n_pipelines, B)
         while B % n_mb:                      # the largest micro-batch count <= n_pipelines that divides the batch
             n_mb -= 1
@@ -859,13 +885,12 @@ class DistributedModel(torch.nn.Module):
         # ---- prefill every micro-batch through the pipeline; the last stage produces the first new token
         multi = self.world > 1
         ring = self._peer_ring(n_mb) if multi else None
-        if multi and ring is None and hasattr(st, "slots"):
+        if multi and ring is None:
             for g in st.slots:                       # NCCL kernels share the SMs during decode: no persistent all-SM kernel
-                if hasattr(g, "allow_chain"):
-                    g.allow_chain = False
+                g.allow_chain = False
         if procs is not None and st.has_head:
             for m in range(n_mb):
-                st.fill_history(m, prompt[m * b:(m + 1) * b].to(dev))
+                st.fill_history(m, req.history[m * b:(m + 1) * b].to(dev))
         if ring is not None:
             if max_new > ring.max_new:
                 raise ValueError(f"max_new_tokens {max_new} exceeds the token log of the peer ring ({ring.max_new})")
@@ -876,10 +901,10 @@ class DistributedModel(torch.nn.Module):
             else:
                 x = torch.empty(b, S, cfg.hidden, dtype=torch.bfloat16, device=dev)
                 link.recv_prev(x)
-            if kv_start is None:
+            if req.kv_start is None:
                 x = st.prefill(x, 0, m)
             else:
-                x = st.prefill(x, 0, m, kv_start=kv_start[m * b:(m + 1) * b])
+                x = st.prefill(x, 0, m, kv_start=req.kv_start[m * b:(m + 1) * b])
             if not link.last:
                 link.send_next(x.clone())
             elif ring is not None:                         # first token straight into the first stage's mailbox
@@ -890,17 +915,15 @@ class DistributedModel(torch.nn.Module):
                 if multi:
                     link.send_up(st.ids_dec[m][:b].clone(), 0)
         if ring is not None:
-            return self._with_scores(self._decode_ring(ring, input_ids, B, S, b, n_mb, max_new, streamer, use_graph, profile, t0),
-                                     S, out)
+            return self._decode_ring(ring, input_ids, req, b, n_mb, t0)
         # ---- decode rounds: micro-batches rotate through the stages; hidden [b,H] hops down, ids hop back up.
         # Sends are asynchronous; a slot's buffer is waited on only right before the next step overwrites it.
         sent_x = [None] * n_mb
         sent_ids = [None] * n_mb
         prof_events = []
-        if profile:
+        if req.profile:
             span = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
             span[0].record()
-        eos_ids = _eos_list(self._eos[0])
         n_cols = max_new
 
         def collect(m, step):
@@ -912,7 +935,7 @@ class DistributedModel(torch.nn.Module):
 
         for step in range(max_new):
             collected = False
-            if eos_ids and step and step % EOS_CHECK_EVERY == 0:
+            if req.eos and step and step % EOS_CHECK_EVERY == 0:
                 # Stop once every row has emitted EOS (HF semantics).  The first stage takes this column's ids of EVERY
                 # micro-batch first, so that no send is left without its posted receive when the ranks meet in the
                 # broadcast below (a collective queued behind an unmatched point-to-point op could wait forever).
@@ -921,7 +944,7 @@ class DistributedModel(torch.nn.Module):
                         collect(m, step)
                 collected = True
                 flag = torch.zeros(1, dtype=torch.int32, device=dev)
-                if link.first and _all_rows_finished(out_tokens[:, :step + 1], eos_ids):
+                if link.first and _all_rows_finished(out_tokens[:, :step + 1], req.eos):
                     flag.fill_(1)
                 if multi:
                     link.flush()
@@ -946,11 +969,11 @@ class DistributedModel(torch.nn.Module):
                     link.recv_prev(st.x_dec[m][:b])
                 if link.last and multi:
                     link.wait(sent_ids[m])
-                if profile:
+                if req.profile:
                     ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
                     ev[0].record()
-                st.decode(m, b, use_graph)
-                if profile:
+                st.decode(m, b, req.use_graph)
+                if req.profile:
                     ev[1].record()
                     prof_events.append(ev)
                 if not link.last:
@@ -958,19 +981,9 @@ class DistributedModel(torch.nn.Module):
                 elif multi:
                     sent_ids[m] = link.send_up(st.ids_dec[m][:b], 0)
         link.flush()
-        if profile:
+        if req.profile:
             span[1].record()
             torch.cuda.synchronize()
             self.timers["decode_span_s"] = span[0].elapsed_time(span[1]) * 1e-3
             self.timers["decode_busy_s"] = sum(a.elapsed_time(b_) for a, b_ in prof_events) * 1e-3
-        if link.first:
-            result = torch.cat([input_ids.to(dev), out_tokens[:, :n_cols]], dim=1)
-        else:
-            result = torch.empty(B, S + n_cols, dtype=torch.int64, device=dev)
-        link.broadcast(result, 0)
-        if hasattr(st, "check"):
-            st.check()
-        if streamer is not None and link.first:
-            streamer.end()
-        self.timers["generate_wall_s"] = time.perf_counter() - t0
-        return self._with_scores(apply_eos(result, S, *self._eos), S, out)
+        return self._finish(req, input_ids, out_tokens, n_cols, t0)

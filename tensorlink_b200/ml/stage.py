@@ -98,12 +98,40 @@ class CudaStage:
 
     def head_logits(self, hidden: torch.Tensor) -> torch.Tensor:
         """final norm + lm_head over [N,H] -> bf16 logits [N,V]."""
+        return self._lm_head(hidden.contiguous())
+
+    def _lm_head(self, hidden: torch.Tensor, logits: Optional[torch.Tensor] = None, hn: Optional[torch.Tensor] = None,
+                 counter: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """final norm + lm_head of [n,H] rows into ``logits`` [n,V] (a new tensor when None): up to gemv_max_rows() rows
+        the GEMV with the norm fused (``counter``: its ticket block), above that the norm into ``hn`` [n,H], then the GEMM."""
         cfg, v = self.cfg, self.params.v
-        n = hidden.shape[0]
-        if n <= gemv_max_rows():
-            return nat.gemv(hidden.contiguous(), v["head"], norm_w=v["norm"], eps=cfg.rms_eps)
-        hn = nat.rmsnorm_fwd(hidden.contiguous(), v["norm"], cfg.rms_eps)
-        return nat.gemm(hn, v["head"])
+        if hidden.shape[0] <= gemv_max_rows():
+            return nat.gemv(hidden, v["head"], out=logits, norm_w=v["norm"], eps=cfg.rms_eps, counter=counter)
+        return nat.gemm(nat.rmsnorm_fwd(hidden, v["norm"], cfg.rms_eps, out=hn), v["head"], out=logits)
+
+    def _pick(self, hidden: torch.Tensor, ids_out: torch.Tensor, logits: torch.Tensor, hn: torch.Tensor,
+              head_ws: torch.Tensor, sample: Optional[tuple] = None, hist: Optional[tuple] = None, log=None):
+        """final norm + lm_head of [n,H] rows into ``logits`` (``_lm_head``), then one token per row into ``ids_out``:
+        the argmax, or with ``sample`` = (sampling dict, counters, sampler workspace, Philox key) a draw from the warped
+        row.  ``hist`` = (log, length, bits, params) of the rows' token histories: both act on HF's processed scores
+        and append the picked id.  ``log``: a score log (``_log``).  Greedy without either, up to gemv_max_rows() rows, is
+        the fused tl_lmhead_argmax (the decode hot path); the others run the GEMV and the picking kernel as two calls."""
+        cfg, v = self.cfg, self.params.v
+        if sample is None and hist is None and log is None and hidden.shape[0] <= gemv_max_rows():
+            nat.lmhead_argmax(hidden, v["head"], v["norm"], cfg.rms_eps, ids_out, logits, head_ws, self.head_ctr)
+            return
+        self._lm_head(hidden, logits, hn, self.head_ctr)
+        if sample is None and hist is None:
+            nat.argmax_bf16(logits, ids_out, head_ws, log=log)
+        elif sample is None:
+            nat.argmax_proc(logits, ids_out, *hist, self.lp_ws, self.lp_flags, score_log=log)
+        else:
+            s, ctr, ws, key = sample
+            warp = (s["temperature"], s["top_k"], s["top_p"])
+            if hist is None:
+                nat.sample(logits, ids_out, ctr, ws, *warp, key, log=log)
+            else:
+                nat.sample_proc(logits, ids_out, *hist, ctr, self.lp_ws, *warp, key, self.lp_flags, score_log=log)
 
     def set_sampling(self, sampling: Optional[dict]):
         """None = greedy.  Changing the mode drops the captured decode graphs (the launch sequence differs)."""
@@ -196,50 +224,10 @@ class CudaStage:
         """next token for [B,H] rows -> ids_out [B] int64: greedy (bit-exact target: torch.argmax of bf16 logits) or, after
         ``set_sampling``, one draw per row from the warped distribution (csrc/sample.cu).  With logits processors on, both
         act on HF's processed scores and append the picked id to the row's history."""
-        log = self._log(slot, hidden.shape[0])
-        if self.procs is not None:
-            self._head_processed(hidden, ids_out, slot, log)
-            return
-        self._head_greedy(hidden, ids_out, log if self.sampling is None else None)
-        if self.sampling is not None:
-            B = hidden.shape[0]
-            s = self.sampling
-            nat.sample(self.logits_dec[:B], ids_out, self.sample_ctr[slot], self.sample_ws, s["temperature"], s["top_k"], s["top_p"],
-                       s["seed"] + 0x9E3779B97F4A7C15 * slot, log=log)
-
-    def _head_processed(self, hidden: torch.Tensor, ids_out: torch.Tensor, slot: int, log=None):
-        cfg, v = self.cfg, self.params.v
-        B = hidden.shape[0]
-        logits = self.logits_dec[:B]
-        if B <= gemv_max_rows():
-            nat.gemv(hidden, v["head"], out=logits, norm_w=v["norm"], eps=cfg.rms_eps,     # the logits tl_lmhead_argmax makes
-                     counter=self.head_ctr)
-        else:
-            nat.rmsnorm_fwd(hidden, v["norm"], cfg.rms_eps, out=self.hn[:B])
-            nat.gemm(self.hn[:B], v["head"], out=logits)
-        hist = (self.hist_log[slot], self.hist_len[slot], self.hist_bits[slot], self.lp_params)
-        if self.sampling is None:
-            nat.argmax_proc(logits, ids_out, *hist, self.lp_ws, self.lp_flags, score_log=log)
-        else:
-            s = self.sampling
-            nat.sample_proc(logits, ids_out, *hist, self.sample_ctr[slot], self.lp_ws, s["temperature"], s["top_k"], s["top_p"],
-                            s["seed"] + 0x9E3779B97F4A7C15 * slot, self.lp_flags, score_log=log)
-
-    def _head_greedy(self, hidden: torch.Tensor, ids_out: torch.Tensor, log=None):
-        """``log``: a score log (``_log``): the argmax logs the logits it reads (tl_lmhead_argmax's two halves, the GEMV
-        and the argmax, run as separate calls then; the same launches)."""
-        cfg, v = self.cfg, self.params.v
-        B = hidden.shape[0]
-        if B <= gemv_max_rows() and log is None:
-            nat.lmhead_argmax(hidden, v["head"], v["norm"], cfg.rms_eps, ids_out, self.logits_dec[:B], self.head_ws,
-                              self.head_ctr)
-            return
-        if B <= gemv_max_rows():
-            nat.gemv(hidden, v["head"], out=self.logits_dec[:B], norm_w=v["norm"], eps=cfg.rms_eps, counter=self.head_ctr)
-        else:
-            nat.rmsnorm_fwd(hidden, v["norm"], cfg.rms_eps, out=self.hn[:B])
-            nat.gemm(self.hn[:B], v["head"], out=self.logits_dec[:B])
-        nat.argmax_bf16(self.logits_dec[:B], ids_out, self.head_ws, log=log)
+        B, s = hidden.shape[0], self.sampling
+        sample = None if s is None else (s, self.sample_ctr[slot], self.sample_ws, stream_seed(s["seed"], slot))
+        hist = None if self.procs is None else (self.hist_log[slot], self.hist_len[slot], self.hist_bits[slot], self.lp_params)
+        self._pick(hidden, ids_out, self.logits_dec[:B], self.hn[:B], self.head_ws, sample, hist, self._log(slot, B))
 
     # ------------------------------------------------------------------------------------------ decode step
     def _decode_body_ring(self, slot: int, B: int, ring):
@@ -281,34 +269,48 @@ class CudaStage:
             return
         ragged = self.slots[slot].ragged          # the captured launches differ (the _rows kernels, no decode chain)
         key = (slot, B, ragged, self.log_mode if self.has_head else None) + (() if ring is None else (id(ring),))
+        # (the warm-up runs without the ring: it must never touch the mailboxes)
+        self._replay(key, lambda: self._decode_body(slot, B, ring), lambda: self._decode_body(slot, B), slot)
+
+    def _step_state(self, slot: int) -> List[torch.Tensor]:
+        """Every piece of device state a decode or verify step of ``slot`` moves: cache position and length, the step's
+        ids / hidden buffers, the sampler counters, the token histories, the score-log columns, the verify step's
+        counters and the assistant's position and length.  A graph's warm-up restores all of them (restoring one the
+        step does not touch is harmless; a missed one would corrupt the first replay)."""
+        grp = self.slots[slot]
+        state = [grp.pos_dev, grp.kvlen_dev, self.ids_dec[slot], self.x_dec[slot]]
+        if not self.has_head:
+            return state
+        state.append(self.sample_ctr)
+        if self.hist_len is not None:
+            state += [self.hist_len, self.hist_bits]
+        if self.score_log is not None:
+            state.append(self.score_log["col"])
+        if self.pl is not None:
+            state += [self.pl[k] for k in ("count", "in_ids", "n_cand", "ctr") if k in self.pl]
+        if self.pl_assistant is not None:
+            state += [self.pl_assistant.slots[0].pos_dev, self.pl_assistant.slots[0].kvlen_dev]
+        return state
+
+    def _replay(self, key, body, warm_up, slot: int):
+        """Replay the graph of ``key``, capturing ``body`` first if there is none: ``warm_up`` runs once outside capture
+        (first-use attribute setting, tensor-map caches), then every tensor of ``_step_state(slot)`` gets its value
+        back, so the warm-up consumes no draw, joins no history and logs no column.  Capture does not execute."""
         g = self.graphs.get(key)
         if g is None:
-            # warm up outside capture (first-use attribute setting, tensor-map cache), restoring the state it touches
-            grp = self.slots[slot]
-            saved = (grp.pos_dev.clone(), grp.kvlen_dev.clone(), self.ids_dec[slot].clone(), self.x_dec[slot].clone())
-            ctr_saved = self.sample_ctr.clone() if self.has_head else None      # the warm-up step must not consume a draw
-            hist_saved = None                                                   # ... nor join a row's token history
-            if self.has_head and self.procs is not None:
-                hist_saved = (self.hist_len.clone(), self.hist_bits.clone())
-            col_saved = self.score_log["col"].clone() if self.has_head and any(self.log_mode) else None  # ... nor a column
+            state = self._step_state(slot)
+            saved = [t.clone() for t in state]
             side = torch.cuda.Stream(device=self.device)
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
-                self._decode_body(slot, B)
+                warm_up()
             torch.cuda.current_stream().wait_stream(side)
-            grp.pos_dev.copy_(saved[0]); grp.kvlen_dev.copy_(saved[1])
-            self.ids_dec[slot].copy_(saved[2]); self.x_dec[slot].copy_(saved[3])
-            if ctr_saved is not None:
-                self.sample_ctr.copy_(ctr_saved)
-            if hist_saved is not None:
-                self.hist_len.copy_(hist_saved[0]); self.hist_bits.copy_(hist_saved[1])
-            if col_saved is not None:
-                self.score_log["col"].copy_(col_saved)
+            for t, s in zip(state, saved):
+                t.copy_(s)
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._decode_body(slot, B, ring)      # (the warm-up above never touches the mailboxes)
-            # capture does not execute; state is still the saved one
+                body()
             self.graphs[key] = g
         g.replay()
 
@@ -388,28 +390,16 @@ class CudaStage:
             pl["n_cand"].fill_(K)
         elif draft:
             nat.pl_draft(log, length, pl["params"], K, pl["in_ids"], pl["n_cand"])
-        x, ids = pl["x"][:n], pl["ids"][:n]
+        x, ids, logits = pl["x"][:n], pl["ids"][:n], pl["logits"][:n]
         nat.embed_fwd(pl["in_ids"][:n], v["embed"], out=x)
         grp.verify_step_inplace(x)
-        if s is not None:
-            logits = pl["logits"][:n]
-            if n <= gemv_max_rows():
-                nat.gemv(x, v["head"], out=logits, norm_w=v["norm"], eps=cfg.rms_eps, counter=self.head_ctr)
-            else:
-                nat.rmsnorm_fwd(x, v["norm"], cfg.rms_eps, out=pl["hn"][:n])
-                nat.gemm(pl["hn"][:n], v["head"], out=logits)
-            warp = (s["temperature"], s["top_k"], s["top_p"])
-            if asst is None:
-                nat.sample(logits, ids, pl["ctr"][:n], pl["sample_ws"], *warp, stream_seed(s["seed"], STREAM_PL_ROWS))
-            else:
-                nat.spec_accept(logits, asst.asst["q"][:K], pl["in_ids"], pl["n_cand"], pl["ctr"][CTR_ACCEPT:CTR_ACCEPT + 1],
-                                ids, pl["spec_ws"], *warp, stream_seed(s["seed"], STREAM_ACCEPT))
-        elif n <= gemv_max_rows():
-            nat.lmhead_argmax(x, v["head"], v["norm"], cfg.rms_eps, ids, pl["logits"][:n], pl["head_ws"], self.head_ctr)
+        if s is not None and asst is not None:
+            self._lm_head(x, logits, pl["hn"][:n], self.head_ctr)
+            nat.spec_accept(logits, asst.asst["q"][:K], pl["in_ids"], pl["n_cand"], pl["ctr"][CTR_ACCEPT:CTR_ACCEPT + 1],
+                            ids, pl["spec_ws"], s["temperature"], s["top_k"], s["top_p"], stream_seed(s["seed"], STREAM_ACCEPT))
         else:
-            nat.rmsnorm_fwd(x, v["norm"], cfg.rms_eps, out=pl["hn"][:n])
-            nat.gemm(pl["hn"][:n], v["head"], out=pl["logits"][:n])
-            nat.argmax_bf16(pl["logits"][:n], ids, pl["head_ws"])
+            sample = None if s is None else (s, pl["ctr"][:n], pl["sample_ws"], stream_seed(s["seed"], STREAM_PL_ROWS))
+            self._pick(x, ids, logits, pl["hn"][:n], pl["head_ws"], sample)
         nat.pl_accept(ids, pl["in_ids"], pl["n_cand"], log, length, bits, cfg.vocab, pl["params"], pl["out_log"], pl["count"],
                       grp.pos_dev, grp.kvlen_dev, K)
 
@@ -421,29 +411,7 @@ class CudaStage:
             return
         asst, sampled = self.pl_assistant, self.sampling is not None
         key = ("verify", self.pl_K + 1, sampled) if asst is None else ("assist", self.pl_K + 1, asst, sampled)
-        g = self.graphs.get(key)
-        if g is None:
-            # warm up outside capture (first-use buffers, attributes), restoring what it touches
-            grp, pl = self.slots[0], self.pl
-            state = (grp.pos_dev, grp.kvlen_dev, pl["count"], pl["in_ids"], pl["n_cand"], self.hist_len, self.hist_bits)
-            if asst is not None:
-                state += (asst.slots[0].pos_dev, asst.slots[0].kvlen_dev)
-            if sampled:
-                state += (pl["ctr"],)                # the warm-up step must not consume a draw
-            saved = [t.clone() for t in state]
-            side = torch.cuda.Stream(device=self.device)
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._verify_body()
-            torch.cuda.current_stream().wait_stream(side)
-            for t, s in zip(state, saved):
-                t.copy_(s)
-            torch.cuda.synchronize(self.device)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._verify_body()
-            self.graphs[key] = g
-        g.replay()
+        self._replay(key, self._verify_body, self._verify_body, 0)
 
     def prompt_lookup_count(self) -> int:
         """Tokens in the output log (synchronises with the device)."""
@@ -501,12 +469,11 @@ class CudaStage:
 
         def head(h, out, i):
             if sample is None:
-                self._head_greedy(h, out)
-                return
-            s, ctr = sample
-            q = a["q"][i:i + 1]
-            nat.gemv(h, v["head"], out=q, norm_w=v["norm"], eps=self.cfg.rms_eps, counter=self.head_ctr)
-            nat.sample(q, out, ctr, a["ws"], s["temperature"], s["top_k"], s["top_p"], stream_seed(s["seed"], STREAM_DRAFTS))
+                self._pick(h, out, self.logits_dec[:1], self.hn[:1], self.head_ws)
+            else:
+                s, ctr = sample
+                self._pick(h, out, a["q"][i:i + 1], self.hn[:1], self.head_ws,
+                           (s, ctr, a["ws"], stream_seed(s["seed"], STREAM_DRAFTS)))
 
         nat.assist_prep(log, length, a["in"], in_ids, grp.pos_dev, grp.kvlen_dev)      # pos = kv_len = P-1
         nat.embed_fwd(a["in"], v["embed"], out=a["x"])

@@ -37,8 +37,8 @@ def test_stage_without_kv_start_takes_the_grouped_path():
     dm.link, dm.stage, dm.cfg, dm.world = _Link(), _Stage(), None, 1
     seen = {}
 
-    def grouped(input_ids, groups, shape, max_new, streamer, use_graph, sampling):
-        seen.update(groups=groups, shape=shape)
+    def grouped(input_ids, req):
+        seen.update(groups=req.groups, shape=req.shape)
         return "grouped"
 
     dm._generate_left_padded = grouped
@@ -52,7 +52,7 @@ def test_stage_without_kv_start_takes_the_grouped_path():
     try:
         got = {}
         dm._generate_left_padded = lambda *a, **k: pytest.fail("a stage with supports_kv_start runs the batch once")
-        dm._generate_batch = lambda input_ids, *a: (got.update(ids=input_ids, kv_start=a[-1]), input_ids)[1]
+        dm._generate_batch = lambda input_ids, req: (got.update(ids=input_ids, kv_start=req.kv_start), input_ids)[1]
         mask = torch.tensor([[0, 0, 1, 1], [0, 1, 1, 1]])
         out = dm.generate(ids, attention_mask=mask, max_new_tokens=2)
         assert got["kv_start"] == [1, 0] and torch.equal(got["ids"], ids[:, 1:])

@@ -106,8 +106,8 @@ def test_history_keeps_the_dropped_pad_columns():
     dm = _dm(_ProcStage())
     seen = {}
 
-    def run(input_ids, max_new, streamer, use_graph, profile, sampling, procs, kv_start):
-        seen.update(ids=input_ids, kv_start=kv_start, procs=procs)
+    def run(input_ids, req):
+        seen.update(ids=input_ids, kv_start=req.kv_start, procs=req.procs, history=req.history)
         return input_ids
 
     dm._generate_batch = run
@@ -115,7 +115,7 @@ def test_history_keeps_the_dropped_pad_columns():
     mask = torch.tensor([[0, 0, 1, 1], [0, 1, 1, 1]])
     dm.generate(ids, attention_mask=mask, max_new_tokens=2, repetition_penalty=1.3)
     assert torch.equal(seen["ids"], ids[:, 1:]) and seen["kv_start"] == [1, 0]
-    prompt = seen["procs"].pop("history")
+    prompt = seen["history"]
     assert seen["procs"] == {"penalty": 1.3, "ngram": 0, "min_new": 0, "eos": []}
     assert torch.equal(prompt, ids)                           # HF counts every column, the pad in every row included
     dm.generate(ids, max_new_tokens=2)

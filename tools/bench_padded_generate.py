@@ -51,19 +51,17 @@ def bench(name, rounds):
     mask = torch.zeros(B, S, dtype=torch.int64)
     for b, L in enumerate(LENGTHS):
         mask[b, S - L:] = 1
-    groups = M._left_pad_groups(mask)
+    req = M._Request(NEW, (B, S), groups=M._left_pad_groups(mask))
     runs = {
         "one_run": lambda: dm.generate(ids, attention_mask=mask, max_new_tokens=NEW),
-        "grouped": lambda: dm._generate_left_padded(ids, groups, (B, S), NEW, None, True, None),
+        "grouped": lambda: dm._generate_left_padded(ids, req),
         "uniform": lambda: dm.generate(ids, max_new_tokens=NEW),
     }
     for fn in runs.values():                      # warm-up: graph capture, tensor maps, first-use attributes
-        dm._eos = (None, None)
         fn()
     times = {k: [] for k in runs}
     for _ in range(rounds):
         for k, fn in runs.items():
-            dm._eos = (None, None)
             out, dt = _timed(fn)
             assert out.shape == (B, S + NEW), (k, out.shape)
             times[k].append(dt)
