@@ -345,6 +345,10 @@ typedef struct tl_decode_job {
 } tl_decode_job;
 /* bytes of the attention-partials workspace shared by every chain launch of a stage */
 size_t tl_decode_chain_ws(int M, int n_h, int n_kv, int d);
+/* host only: the shared-memory ring tl_decode_chain builds for M rows whose widest GEMV job has K = k_max.  stage_kb < 0
+ * takes the process's TL_CHAIN_STAGE_KB (what tl_decode_chain uses), 0 the default geometry, > 0 forces a slot size.
+ * out[4] = {slot bytes, slots, consumer warps NW, K chunk}; TL_ERR_INVALID when the launcher cannot place the shape. */
+int tl_decode_chain_geometry(int M, int k_max, int stage_kb, int* out);
 /* jobs: HOST array (copied into kernel parameter space).  sync_slot: TL_DECODE_CHAIN_SYNC_BYTES of device memory
  * private to this launch site (consecutive launches under programmatic dependent launch must not share one); word 2
  * is an error flag the kernel raises instead of hanging when a dependency wait exceeds 2 s.  pf_ptr/pf_bytes:

@@ -834,6 +834,51 @@ size_t tl_decode_chain_ws(int M, int n_h, int n_kv, int d) {
     return (size_t)M * n_h * cpg * (d + 4) * sizeof(float) + 256;
 }
 
+static int chain_stage_kb() {       // TL_CHAIN_STAGE_KB, read once (any value below 8 but 0 forces 16 KB slots)
+    static int forced_kb = -1;
+    if (forced_kb < 0) {
+        const char* e = getenv("TL_CHAIN_STAGE_KB");
+        forced_kb = e ? atoi(e) : 0;
+        if (forced_kb < 0) forced_kb = 16;
+    }
+    return forced_kb;
+}
+
+int tl_decode_chain_geometry(int M, int k_max, int stage_kb, int* out) {
+    using namespace tl;
+    TL_REQUIRE(M >= 1 && M <= DC_MAX_M && k_max >= 0 && out, TL_ERR_INVALID, "tl_decode_chain_geometry: M=%d k_max=%d", M, k_max);
+    const int forced_kb = stage_kb < 0 ? chain_stage_kb() : stage_kb;
+    constexpr int SMEM_CAP = 227 * 1024 - 1024;       // static shared memory of the kernel stays below 1 KB
+    const size_t xs_bytes = (((size_t)M * k_max * 2) + 127) & ~(size_t)127;
+    const size_t fixed = xs_bytes + (size_t)DC_ATTN_BYTES + 2 * DC_MAX_STAGES * sizeof(uint64_t);
+    // The consumers are the scarce resource (one warp per scheduler cannot hide its own latencies), so all 8 consumer
+    // warps get a slot class of their own: 8 slots (n_stages % NW == 0: a slot is always drained by the same warp) as
+    // large as shared memory allows, capped at 24 KB.  Below 12 KB per slot, or with a forced slot size, as many slots
+    // as fit, NW = the largest divisor-compatible warp count.
+    int DC_STAGE = 0, n_stages = 0, NW = 0;
+    TL_REQUIRE(fixed + 4 * 8192 <= (size_t)SMEM_CAP, TL_ERR_INVALID, "tl_decode_chain: M*K_max too large (%zu B fixed)", fixed);
+    if (!forced_kb) {
+        int kb = (int)((SMEM_CAP - fixed) / 8 / 1024);
+        if (kb > 24) kb = 24;
+        if (kb >= 12) { DC_STAGE = kb * 1024; n_stages = 8; NW = 8; }
+    }
+    if (!DC_STAGE) {
+        DC_STAGE = (forced_kb >= 8 ? forced_kb : 16) * 1024;
+        int max_stages = (int)((SMEM_CAP - fixed) / DC_STAGE);
+        if (max_stages > DC_MAX_STAGES) max_stages = DC_MAX_STAGES;
+        TL_REQUIRE(max_stages >= 4, TL_ERR_INVALID, "tl_decode_chain: fewer than 4 ring slots fit");
+        for (int nw = DC_CW; nw >= 4; --nw) {
+            const int st_ = max_stages / nw * nw;
+            if (st_ > n_stages) { n_stages = st_; NW = nw; }
+        }
+    }
+    out[0] = DC_STAGE;
+    out[1] = n_stages;
+    out[2] = NW;
+    out[3] = (DC_STAGE / 4) & ~7;
+    return TL_OK;
+}
+
 int tl_decode_chain(const tl_decode_job* jobs, int n_jobs, int M, void* sync_slot, void* attn_ws, size_t attn_ws_bytes,
                     const void* pf_ptr, size_t pf_bytes, void* stream) {
     using namespace tl;
@@ -862,36 +907,12 @@ int tl_decode_chain(const tl_decode_job* jobs, int n_jobs, int M, void* sync_slo
         }
     }
     (void)n_attn;
-    constexpr int SMEM_CAP = 227 * 1024 - 1024;       // static shared memory of the kernel stays below 1 KB
+    constexpr int SMEM_CAP = 227 * 1024 - 1024;
     const size_t xs_bytes = (((size_t)M * k_max * 2) + 127) & ~(size_t)127;
-    const size_t attn_bytes = (size_t)DC_ATTN_BYTES;
-    const size_t fixed = xs_bytes + attn_bytes + 2 * DC_MAX_STAGES * sizeof(uint64_t);
-    // Ring geometry.  The consumers are the scarce resource (one warp per scheduler cannot hide its own latencies), so all 8 consumer warps get a slot class of their own: 8 slots (n_stages % NW == 0:
-    // a slot is always drained by the same warp) as large as shared memory allows, capped at 24 KB.  TL_CHAIN_STAGE_KB
-    // forces a slot size (then as many slots as fit, NW = the largest divisor-compatible warp count).
-    static int forced_kb = -1;
-    if (forced_kb < 0) {
-        const char* e = getenv("TL_CHAIN_STAGE_KB");
-        forced_kb = e ? atoi(e) : 0;
-    }
-    int DC_STAGE = 0, n_stages = 0, NW = 0;
-    TL_REQUIRE(fixed + 4 * 8192 <= (size_t)SMEM_CAP, TL_ERR_INVALID, "tl_decode_chain: M*K_max too large (%zu B fixed)", fixed);
-    if (!forced_kb) {
-        int kb = (int)((SMEM_CAP - fixed) / 8 / 1024);
-        if (kb > 24) kb = 24;
-        if (kb >= 12) { DC_STAGE = kb * 1024; n_stages = 8; NW = 8; }
-    }
-    if (!DC_STAGE) {
-        DC_STAGE = (forced_kb >= 8 ? forced_kb : 16) * 1024;
-        int max_stages = (int)((SMEM_CAP - fixed) / DC_STAGE);
-        if (max_stages > DC_MAX_STAGES) max_stages = DC_MAX_STAGES;
-        TL_REQUIRE(max_stages >= 4, TL_ERR_INVALID, "tl_decode_chain: fewer than 4 ring slots fit");
-        for (int nw = DC_CW; nw >= 4; --nw) {
-            const int st_ = max_stages / nw * nw;
-            if (st_ > n_stages) { n_stages = st_; NW = nw; }
-        }
-    }
-    const int DC_KC = (DC_STAGE / 4) & ~7;
+    const size_t fixed = xs_bytes + (size_t)DC_ATTN_BYTES + 2 * DC_MAX_STAGES * sizeof(uint64_t);
+    int geo[4];
+    if (tl_decode_chain_geometry(M, k_max, -1, geo) != TL_OK) return TL_ERR_INVALID;
+    const int DC_STAGE = geo[0], n_stages = geo[1], NW = geo[2], DC_KC = geo[3];
     ChainParams prm = {};
     prm.n_jobs = n_jobs;
     prm.n_stages = n_stages;

@@ -579,7 +579,14 @@ class CudaLayerGroup:
         return (os.environ.get("TL_DECODE_IMPL", "kernels") == "chain" and self.allow_chain and self.num_layers > 0
                 and not self.ragged and not self.p.fp8
                 and B <= min(4, gemv_max_rows()) and cfg.n_kv_heads * B <= 60 and cfg.n_heads // cfg.n_kv_heads <= 8
-                and cfg.head_dim in (64, 128))
+                and cfg.head_dim in (64, 128) and self._chain_ring_fits(B))
+
+    def _chain_ring_fits(self, B: int) -> bool:
+        """The chain launcher places B rows of the widest input (the down projection's) beside its weight ring; at
+        Qwen2.5-7B width four rows leave too little shared memory for the ring, and such steps take the per-kernel
+        sequence."""
+        cfg = self.cfg
+        return nat.decode_chain_geometry(B, max(cfg.hidden, cfg.q_dim, cfg.intermediate)) is not None
 
     def _chain_group(self) -> int:
         """Decoder layers per chain launch (TL_CHAIN_LAYERS, default 1; 5 jobs per layer, at most 3 layers)."""
@@ -643,7 +650,7 @@ class CudaLayerGroup:
         long and a short weight stream)."""
         import os
         return (os.environ.get("TL_DECODE_IMPL", "kernels") == "dq" and self.allow_chain and self.num_layers > 1
-                and B <= min(4, gemv_max_rows()) and not self.p.fp8)
+                and B <= min(4, gemv_max_rows()) and not self.p.fp8 and self._chain_ring_fits(B))
 
     def _decode_step_dq(self, x: torch.Tensor, B: int, out: Optional[torch.Tensor]):
         cfg, v = self.cfg, self.p.v

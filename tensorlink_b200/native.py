@@ -74,6 +74,7 @@ _SIGS = {
     "tl_attn_decode_fused_rows": (c_int, [c_void_p] * 9 + [c_float, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p,
                                                            c_void_p]),
     "tl_decode_chain_ws": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "tl_decode_chain_geometry": (c_int, [c_int, c_int, c_int, c_void_p]),
     "tl_decode_chain_trace": (c_int, [c_void_p, c_int]),
     "tl_decode_chain": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),
     "tl_peer_alloc": (c_int, [c_size_t, POINTER(c_void_p), c_void_p]),
@@ -846,6 +847,15 @@ def attn_decode_fused(qkv, k_cache, v_cache, out, pos_dev, cos_tab, sin_tab, q_n
 
 def decode_chain_ws(M: int, n_h: int, n_kv: int, d: int) -> int:
     return int(load().tl_decode_chain_ws(M, n_h, n_kv, d))
+
+
+def decode_chain_geometry(M: int, k_max: int, stage_kb: int = -1) -> Optional[tuple]:
+    """(slot bytes, slots, consumer warps, K chunk) of the ring tl_decode_chain builds for M rows and a widest GEMV
+    K of k_max, or None when it cannot place that shape.  stage_kb < 0: the process's TL_CHAIN_STAGE_KB.  Host only."""
+    out = (ctypes.c_int * 4)()
+    if load().tl_decode_chain_geometry(M, k_max, stage_kb, ctypes.cast(out, c_void_p)) != 0:
+        return None
+    return tuple(out)
 
 
 CHAIN_TRACE_WORDS = 2 * (CHAIN_MAX_JOBS + 1) * 4 + CHAIN_MAX_JOBS * 160 + CHAIN_MAX_JOBS * 4

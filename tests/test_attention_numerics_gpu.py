@@ -27,17 +27,14 @@ Calibrated on an H100 80GB HBM3 (400 W power limit); worst measured error / boun
   lse 0.24  (LSE_ATOL = 3e-5, LSE_RTOL = 3e-6)
 The mma.sync and wgmma backward give the same worst rows.  The file runs in about 10 s there (216 tests).
 """
-import math
-
 import pytest
 import torch
 
-from oracle import shard_oracle as O
 from tests import attn_patterns as P
+from tests.attn_patterns import FWD_FLOOR, FWD_K, check_rows, oracle_fwd, ref_fwd
 
 pytestmark = pytest.mark.gpu
 
-FWD_K, FWD_FLOOR = 2.0, 2e-3
 BWD_K, BWD_FLOOR, BWD_CANCEL = 2.0, 2e-3, 8e-3
 LSE_ATOL, LSE_RTOL = 3e-5, 3e-6
 NAN = float("nan")
@@ -51,20 +48,6 @@ def nat():
 
 
 # ------------------------------------------------------------------------------------------ float64 references
-def ref_fwd(q, k, v, past, scale):
-    """Causal GQA attention in float64: q [B,S,n_h,d], k/v [B,n_kv,T,d] (bf16, on the GPU), queries at positions
-    past..past+S-1.  Returns out [B,S,n_h,d] and lse [B,n_h,S] (natural log)."""
-    B, S, n_h, d = q.shape
-    T, n_rep = k.shape[2], n_h // k.shape[1]
-    kk, vv = k.double().repeat_interleave(n_rep, 1), v.double().repeat_interleave(n_rep, 1)
-    s = (q.double().transpose(1, 2) @ kk.transpose(2, 3)) * scale
-    above = torch.arange(T, device=q.device)[None, :] > torch.arange(past, past + S, device=q.device)[:, None]
-    s.masked_fill_(above, float("-inf"))
-    lse = torch.logsumexp(s, -1)
-    out = torch.exp(s - lse[..., None]) @ vv
-    return out.transpose(1, 2), lse
-
-
 def ref_bwd(q, k, v, do, scale):
     """Gradients of causal GQA attention (past = 0) in float64 for the upstream gradient do [B,S,n_h,d]:
     dq [B,S,n_h,d], dk and dv [B,n_kv,S,d] (summed over each group's query heads).  Also the same products taken over
@@ -84,13 +67,6 @@ def ref_bwd(q, k, v, do, scale):
     grads = ((ds @ kk).transpose(1, 2), group(ds.transpose(2, 3) @ qd), group(p.transpose(2, 3) @ dod))
     sizes = ((dsa @ kk.abs()).transpose(1, 2), group(dsa.transpose(2, 3) @ qd.abs()), group(p.transpose(2, 3) @ dod.abs()))
     return grads, sizes
-
-
-def oracle_fwd(q, k, v, scale):
-    """The bf16 yardstick: O.attention_sdpa_math on the CPU (queries are the last S positions of k / v)."""
-    n_rep = q.shape[2] // k.shape[1]
-    o = O.attention_sdpa_math(q.cpu().transpose(1, 2), k.cpu(), v.cpu(), scale, n_rep)
-    return o.view(q.shape)
 
 
 def oracle_bwd(q, k, v, do, scale):
@@ -115,30 +91,6 @@ def oracle_bwd(q, k, v, do, scale):
 
 
 # ------------------------------------------------------------------------------------------ criteria
-def row_errors(got, ref, oracle, size=None):
-    """Per-row distances to float64 of the kernel and of the oracle; the RMS row norm of the reference and of `size`
-    (same shape, or None) within each batch row (the batch rows differ in magnitude on purpose).  Tensors have the
-    batch as their first dim."""
-    B, d = ref.shape[0], ref.shape[-1]
-    rows = lambda x: x.reshape(B, -1, d).to(ref.device, torch.float64)
-    rms = lambda x: x.pow(2).sum(-1).mean(-1, keepdim=True).sqrt().expand(B, x.shape[1]).flatten()
-    r = rows(ref)
-    e_k = (rows(got) - r).norm(dim=-1).flatten()
-    e_o = (rows(oracle) - r).norm(dim=-1).flatten()
-    return e_k, e_o, rms(r), rms(rows(size)) if size is not None else torch.zeros_like(e_k)
-
-
-def check_rows(what, got, ref, oracle, k, floor, size=None, cancel=0.0):
-    """Each row: |got - ref| <= k |oracle - ref| + floor * RMS(ref) + cancel * RMS(size)."""
-    assert bool(torch.isfinite(got).all()), f"{what}: {int((~torch.isfinite(got)).sum())} non-finite values"
-    e_k, e_o, rms, rms_size = row_errors(got, ref, oracle, size)
-    bound = k * e_o + floor * rms + cancel * rms_size
-    ratio = e_k / bound
-    worst = int(ratio.argmax())
-    assert float(ratio[worst]) <= 1.0, (f"{what}: row {worst} (of {ratio.numel()}) error {float(e_k[worst]):.3e} > bound "
-                                        f"{float(bound[worst]):.3e} ({k} x oracle {float(e_o[worst]):.3e} + floors)")
-
-
 def check_lse(what, got, ref):
     assert bool(torch.isfinite(got).all()), f"{what}: non-finite lse"
     err = (got.double() - ref).abs()
@@ -270,10 +222,6 @@ FUSED_GEOM = [(28, 4, 128, False), (14, 2, 64, True), (32, 4, 128, True), (16, 2
 FUSED_PATTERNS = ["flat", "sink", "rising", "falling", "spike@T-1", "spike@T-2", "wide"]
 
 
-def _rms_norm(x, eps):
-    return x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + eps)
-
-
 FUSED_CASES = [(pos, pat) for pos in (0, 1, 255, 2046, 2047) for pat in FUSED_PATTERNS if not (pos == 0 and pat == "spike@T-2")]
 
 
@@ -286,45 +234,9 @@ def test_decode_fused(nat, pos, n_h, n_kv, d, qk_norm, pattern):
     the k-norm gain when the norm is on.  The reference attends with the rotated query and the cache that
     rope_kv_fwd produces, and the fused kernel's cache must equal that one bit for bit."""
     B, eps, scale, T = 2, 1e-6, d ** -0.5, pos + 1
-    n_rep, a = n_h // n_kv, P.designed_dims(d)[0]
-    designed = P.is_designed(pattern)
-    z = P.logit_pattern(pattern, T)
-    std = P.NOISE_STD.get(pattern, P.NOISE_STD_DESIGNED)
-    g = torch.Generator().manual_seed(41 + pos)
-    qkv = torch.randn(B, n_h + 2 * n_kv, d, generator=g) * std
-    qkv[:, n_h + n_kv:] = P.make_v(B, n_kv, 1, d, seed=42 + pos).view(B, n_kv, d).float()
-    qn = kn = None
-    if qk_norm:
-        qn, kn = (1 + 0.1 * torch.randn(d, generator=g)), (1 + 0.1 * torch.randn(d, generator=g))
-    if designed:
-        qkv[:, :n_h, a] = math.sqrt(d)
-        qkv[:, n_h:n_h + n_kv, a] = 1.0
-        if qk_norm:
-            qn[a] = 1.0
-    qkv = qkv.bfloat16()
-    # the query's designed component as the kernel will see it (norm; RoPE leaves it within 4e-3 rad)
-    qa = qkv[:, :n_h].float()
-    if qk_norm:
-        qa = _rms_norm(qa, eps) * qn.bfloat16().float()
-    qa = qa[..., a].view(B, n_kv, n_rep).mean(-1)                     # [B, n_kv]
-    if designed:
-        target = z[pos].item() * math.sqrt(d)                         # wanted k_a of the new key times q_a
-        if qk_norm:
-            kr = _rms_norm(qkv[:, n_h:n_h + n_kv].float(), eps)[..., a].mean().item()
-            kn[a] = target / qa.mean().item() / kr
-        else:
-            qkv[:, n_h:n_h + n_kv, a] = (target / qa).bfloat16()
-    qkv = qkv.reshape(B, -1).cuda()
-    qn = qn.bfloat16().cuda() if qk_norm else None
-    kn = kn.bfloat16().cuda() if qk_norm else None
-    kc0 = torch.full((B, n_kv, FD_T_MAX, d), NAN, dtype=torch.bfloat16)
-    vc0 = torch.full_like(kc0, NAN)
-    if pos:
-        kc0[:, :, :pos] = torch.randn(B, n_kv, pos, d, generator=g) * std
-        if designed:
-            kc0[:, :, :pos, a] = (z[:pos].view(1, 1, pos) * math.sqrt(d) / qa.double()[..., None]).bfloat16()
-        vc0[:, :, :pos] = P.make_v(B, n_kv, pos, d, seed=43 + pos)
-    kc0, vc0 = kc0.cuda(), vc0.cuda()
+    n_rep, designed, z = n_h // n_kv, P.is_designed(pattern), P.logit_pattern(pattern, pos + 1)
+    qkv, qn, kn, kc0, vc0 = (t.cuda() if t is not None else None
+                             for t in P.decode_inputs(pattern, B, pos, n_h, n_kv, d, qk_norm, FD_T_MAX, eps))
     ct, st = nat.rope_table(1.0 / (1e6 ** (torch.arange(0, d, 2, dtype=torch.float32) / d)).cuda(), FD_T_MAX)
     posd = torch.tensor([pos], dtype=torch.int32, device="cuda")
     kc1, vc1 = kc0.clone(), vc0.clone()
