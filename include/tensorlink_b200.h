@@ -218,15 +218,26 @@ int tl_argmax_bf16_log(const void* logits, int64_t* ids_out, void* workspace, si
 /* ---- token sampling on the device (csrc/sample.cu): what HF `generate(do_sample=True)` does on the host's copy of the
  * logits (the reference delegates to it, tensorlink/ml/module.py:763-769, ml/worker.py:403-404): temperature -> top-k
  * (every logit >= the k-th largest is kept; 0 = off) -> top-p (a token is kept while the probability mass above it is
- * < top_p; ties at the threshold are kept) -> one multinomial draw per row from Philox4x32-10(seed; row, counter).
+ * < top_p; ties at the threshold are kept) -> min_p -> typical_p -> epsilon -> eta -> one multinomial draw per row from
+ * Philox4x32-10(seed; row, counter).  The last four arguments are HF's MinP / Typical / Epsilon / Eta warpers
+ * (min_tokens_to_keep 1), each over the set the stages before it kept, p = softmax(x / T) over that set, H its entropy:
+ * min_p keeps p >= min_p * p_max; typical_p = m keeps a group of equal distance |E[x/T] - x/T| while the mass of the
+ * strictly closer tokens is < m (it may drop the top tokens); epsilon keeps p >= epsilon; eta keeps p >=
+ * min(eta, sqrt(eta) * exp(-H)); the last two always keep the set's top value.  Off at min_p 0, typical_p 1, epsilon 0,
+ * eta 0, which run the sampler as without them; 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= epsilon < 1 and
+ * 0 <= eta < 1, else TL_ERR_INVALID.  The kept set is always one interval of values.  The same four arguments act alike
+ * in tl_sample_proc and tl_spec_accept.  They need no more workspace, except tl_spec_accept's 8 bytes per row for the
+ * interval's top.
  * counters_dev: int32[M] in device memory, advanced by the kernel (a captured graph draws a fresh number per replay).
  * workspace >= tl_sample_ws(M) bytes.  logits bf16 [M,V] row-major; ids_out int64[M]. */
 size_t tl_sample_ws(int M);
 int tl_sample(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
-              unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream);
+              unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream, float min_p,
+              float typical_p, float epsilon, float eta);
 int tl_sample_log(const void* logits, int64_t* ids_out, int M, int V, float temperature, int top_k, float top_p,
                   unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, float* raw_log,
-                  float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream);
+                  float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream, float min_p,
+                  float typical_p, float epsilon, float eta);
 /* speculative sampling after a verify pass (Leviathan et al. Algorithm 1, HF _speculative_sampling), one row: the
  * target's rows p_logits bf16 [K+1, V_p] and the assistant's q_logits bf16 [K, V_q], each warped by tl_sample's rules
  * with the same temperature / top_k / top_p; the drafts d_i = in_ids[i+1] for i < n = min(*n_cand, K).  Draft i is kept
@@ -239,7 +250,8 @@ int tl_sample_log(const void* logits, int64_t* ids_out, int M, int V, float temp
 size_t tl_spec_accept_ws(int K);
 int tl_spec_accept(const void* p_logits, int V_p, const void* q_logits, int V_q, int K, const int64_t* in_ids,
                    const int32_t* n_cand, float temperature, int top_k, float top_p, unsigned long long seed,
-                   int32_t* counter_dev, int64_t* ids_out, void* workspace, size_t ws_bytes, void* stream);
+                   int32_t* counter_dev, int64_t* ids_out, void* workspace, size_t ws_bytes, void* stream, float min_p,
+                   float typical_p, float epsilon, float eta);
 
 /* ---- logits processors (csrc/logits_process.cu): HF's RepetitionPenaltyLogitsProcessor -> NoRepeatNGramLogitsProcessor
  * -> MinNewTokensLengthLogitsProcessor on the fp32 copy of the bf16 logits, before the argmax or the warpers above.
@@ -269,7 +281,8 @@ int tl_argmax_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* 
  * probability mass is summed as 64-bit fixed-point integers, so a seed reproduces its tokens) */
 int tl_sample_proc(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
                    const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
-                   unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream);
+                   unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, void* stream, float min_p,
+                   float typical_p, float epsilon, float eta);
 /* the score-log twins (see tl_argmax_bf16_log) */
 int tl_argmax_proc_log(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
                        const int32_t* params_dev, int flags, void* workspace, size_t ws_bytes, int M, int V, int L,
@@ -277,7 +290,8 @@ int tl_argmax_proc_log(const void* logits, int64_t* ids_out, int32_t* log, int32
 int tl_sample_proc_log(const void* logits, int64_t* ids_out, int32_t* log, int32_t* len, uint32_t* bits,
                        const int32_t* params_dev, int flags, int M, int V, int L, float temperature, int top_k, float top_p,
                        unsigned long long seed, int32_t* counters_dev, void* workspace, size_t ws_bytes, float* raw_log,
-                       float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream);
+                       float* score_log, int32_t* log_col, int n_cols, int B_total, int row0, void* stream, float min_p,
+                       float typical_p, float epsilon, float eta);
 
 /* ---- prompt-lookup decoding (csrc/prompt_lookup.cu), one row: a verify step runs in_ids[0..K] (the last history token
  * and K drafts) as K+1 rows and keeps the drafts the model agrees with.  The history is the logits processors' (log, len,

@@ -67,6 +67,26 @@ _NEUTRAL_KW = {"use_cache": (True, False, None), "return_dict": (True, None), "o
                "num_assistant_tokens_schedule": ("constant", None), "assistant_confidence_threshold": (None,)}
 
 
+def _warpers(min_p=None, typical_p=None, epsilon_cutoff=None, eta_cutoff=None) -> dict:
+    """The sampling dict's entries for HF's MinP / Typical / Epsilon / Eta warpers (ml/stage.py WARPER_KEYS), active
+    ones only: as in HF's ``_get_logits_processor``, min_p is off at None or 0, typical_p at None or >= 1, and
+    epsilon_cutoff / eta_cutoff at None or outside (0, 1); the values HF's warpers reject raise ValueError."""
+    out = {}
+    if min_p is not None:
+        if not 0.0 <= float(min_p) <= 1.0:
+            raise ValueError(f"`min_p` has to be a float in the [0, 1] interval, but is {min_p}")
+        if float(min_p) > 0.0:
+            out["min_p"] = float(min_p)
+    if typical_p is not None and float(typical_p) < 1.0:
+        if not float(typical_p) > 0.0:
+            raise ValueError(f"`typical_p` has to be a float > 0 and < 1, but is {typical_p}")
+        out["typical_p"] = float(typical_p)
+    for name, key, v in (("epsilon_cutoff", "epsilon", epsilon_cutoff), ("eta_cutoff", "eta", eta_cutoff)):
+        if v is not None and 0.0 < float(v) < 1.0:
+            out[key] = float(v)
+    return out
+
+
 def _check_unconsumed(kwargs: dict, what: str):
     for k, v in kwargs.items():
         ok = _NEUTRAL_KW.get(k)
@@ -284,7 +304,7 @@ class _Request:
     """One ``generate`` call, parsed once (``DistributedModel._request``) and the same on every rank."""
     max_new: int
     shape: tuple                      # [rows, S] of the prompt the run sees (from the first rank, as those below)
-    sampling: Optional[dict] = None   # {temperature, top_k, top_p, seed}, or None: greedy
+    sampling: Optional[dict] = None   # {temperature, top_k, top_p, seed, + active warpers}, or None: greedy
     eos: tuple = ()                   # the EOS ids
     pad_token_id: Optional[int] = None
     procs: Optional[dict] = None      # _logits_processors
@@ -695,8 +715,12 @@ class DistributedModel(torch.nn.Module):
     def generate(self, *args, **kwargs) -> Optional[torch.Tensor]:
         """Generation (module.py:763-769 delegates to HF ``generate``).  Greedy by default; ``do_sample=True`` draws every
         token on the last stage's GPU from the distribution HF's warpers define — ``temperature`` (default 1.0), ``top_k``
-        (default 50, 0 = off), ``top_p`` (default 1.0) — with a counter-based Philox stream keyed by ``seed`` (extension;
-        default ``torch.initial_seed()``): the same seed reproduces the same tokens (csrc/sample.cu).
+        (default 50, 0 = off), ``top_p`` (default 1.0), then ``min_p``, ``typical_p``, ``epsilon_cutoff`` and ``eta_cutoff``
+        (HF's MinP / Typical / Epsilon / Eta warpers in that order, each off by default; off too at min_p 0, typical_p
+        >= 1 and a cutoff outside (0, 1), as in HF; min_p outside [0, 1] or typical_p <= 0 raises ValueError) — with a
+        counter-based Philox stream keyed by ``seed`` (extension; default ``torch.initial_seed()``): the same seed
+        reproduces the same tokens (csrc/sample.cu).  Every sampled mode below applies all of them.  Greedy, these
+        keywords are ignored, as HF does.  ``top_h`` raises NotImplementedError.
         ``repetition_penalty``, ``no_repeat_ngram_size`` and ``min_new_tokens`` act as HF's logits processors, in that
         order and before the sampling warpers, on the last stage's GPU inside the decode graph (csrc/logits_process.cu).
         As in HF the history they look at is the whole ``input_ids`` row, pad tokens included, plus the generated tokens.
@@ -777,12 +801,14 @@ class DistributedModel(torch.nn.Module):
         profile = kwargs.pop("profile", False)       # CUDA events around every decode launch -> self.timers["decode_busy_s"]
         sampling = None
         temperature, top_k, top_p = kwargs.pop("temperature", None), kwargs.pop("top_k", None), kwargs.pop("top_p", None)
+        warp = {k: kwargs.pop(k, None) for k in ("min_p", "typical_p", "epsilon_cutoff", "eta_cutoff")}
         seed = kwargs.pop("seed", None)
         if kwargs.pop("do_sample", False):
             sampling = {"temperature": 1.0 if temperature is None else float(temperature), "top_k": 50 if top_k is None else int(top_k),
                         "top_p": 1.0 if top_p is None else float(top_p), "seed": int(torch.initial_seed() if seed is None else seed)}
             if sampling["temperature"] <= 0 or not (0 < sampling["top_p"] <= 1) or sampling["top_k"] < 0:
                 raise ValueError(f"invalid sampling parameters {sampling}")
+            sampling.update(_warpers(**warp))
         eos_token_id, pad_token_id = kwargs.pop("eos_token_id", None), kwargs.pop("pad_token_id", None)
         procs = _logits_processors(kwargs.pop("repetition_penalty", None), kwargs.pop("no_repeat_ngram_size", None),
                                    kwargs.pop("min_new_tokens", None), eos_token_id)

@@ -31,6 +31,15 @@ def stream_seed(seed: int, stream: int) -> int:
     return (seed + GOLDEN * stream) & (2 ** 64 - 1)
 
 
+# the sampling dict's optional warpers (generate's min_p / typical_p / epsilon_cutoff / eta_cutoff) as the keyword
+# arguments of nat.sample / sample_proc / spec_accept; a dict carries only the active ones
+WARPER_KEYS = ("min_p", "typical_p", "epsilon", "eta")
+
+
+def warpers(sampling: dict) -> dict:
+    return {k: sampling[k] for k in WARPER_KEYS if k in sampling}
+
+
 class CudaStage:
     def __init__(self, cfg: ShardModelConfig, layer_ids, has_embed: bool, has_head: bool, device,
                  max_batch: int, max_seq: int, n_slots: int = 1, training: bool = False,
@@ -67,6 +76,7 @@ class CudaStage:
             self.hn = torch.empty(max_batch, cfg.hidden, dtype=torch.bfloat16, device=dev)
             self.head_ctr = nat.gemv_counters(device=dev)        # the decode lm_head GEMV's ticket counter
             self.sampling: Optional[dict] = None        # set by generate(do_sample=True): temperature / top_k / top_p / seed
+                                                        # (+ the active WARPER_KEYS)
             self.sample_ctr = torch.zeros(n_slots, max_batch, dtype=torch.int32, device=dev)
             self.sample_ws: Optional[torch.Tensor] = None
             # logits processors (set_logits_processors): per slot and row a token history on the device -- log
@@ -129,9 +139,10 @@ class CudaStage:
             s, ctr, ws, key = sample
             warp = (s["temperature"], s["top_k"], s["top_p"])
             if hist is None:
-                nat.sample(logits, ids_out, ctr, ws, *warp, key, log=log)
+                nat.sample(logits, ids_out, ctr, ws, *warp, key, log=log, **warpers(s))
             else:
-                nat.sample_proc(logits, ids_out, *hist, ctr, self.lp_ws, *warp, key, self.lp_flags, score_log=log)
+                nat.sample_proc(logits, ids_out, *hist, ctr, self.lp_ws, *warp, key, self.lp_flags, score_log=log,
+                                **warpers(s))
 
     def set_sampling(self, sampling: Optional[dict]):
         """None = greedy.  Changing the mode drops the captured decode graphs (the launch sequence differs)."""
@@ -396,7 +407,8 @@ class CudaStage:
         if s is not None and asst is not None:
             self._lm_head(x, logits, pl["hn"][:n], self.head_ctr)
             nat.spec_accept(logits, asst.asst["q"][:K], pl["in_ids"], pl["n_cand"], pl["ctr"][CTR_ACCEPT:CTR_ACCEPT + 1],
-                            ids, pl["spec_ws"], s["temperature"], s["top_k"], s["top_p"], stream_seed(s["seed"], STREAM_ACCEPT))
+                            ids, pl["spec_ws"], s["temperature"], s["top_k"], s["top_p"], stream_seed(s["seed"], STREAM_ACCEPT),
+                            **warpers(s))
         else:
             sample = None if s is None else (s, pl["ctr"][:n], pl["sample_ws"], stream_seed(s["seed"], STREAM_PL_ROWS))
             self._pick(x, ids, logits, pl["hn"][:n], pl["head_ws"], sample)

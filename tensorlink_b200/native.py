@@ -25,6 +25,7 @@ class NativeError(RuntimeError):
 # the trailing arguments of the score-log (_log) entry points: raw log, score log, column counter, n_cols, B_total, row0,
 # stream
 _LOG_ARGS = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]
+_WARP_ARGS = [c_float, c_float, c_float, c_float]      # min_p, typical_p, epsilon, eta
 
 _SIGS = {
     "tl_abi_version": (c_int, []),
@@ -91,20 +92,20 @@ _SIGS = {
     "tl_argmax_bf16_log": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int] + _LOG_ARGS),
     "tl_sample_ws": (c_size_t, [c_int]),
     "tl_sample": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p, c_void_p, c_size_t,
-                          c_void_p]),
+                          c_void_p] + _WARP_ARGS),
     "tl_sample_log": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p, c_void_p,
-                              c_size_t] + _LOG_ARGS),
+                              c_size_t] + _LOG_ARGS + _WARP_ARGS),
     "tl_spec_accept_ws": (c_size_t, [c_int]),
     "tl_spec_accept": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_float,
-                               ctypes.c_uint64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+                               ctypes.c_uint64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p] + _WARP_ARGS),
     "tl_logits_proc_ws": (c_size_t, [c_int, c_int]),
     "tl_history_fill": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "tl_argmax_proc": (c_int, [c_void_p] * 6 + [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
     "tl_sample_proc": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p,
-                                                c_void_p, c_size_t, c_void_p]),
+                                                c_void_p, c_size_t, c_void_p] + _WARP_ARGS),
     "tl_argmax_proc_log": (c_int, [c_void_p] * 6 + [c_int, c_void_p, c_size_t, c_int, c_int, c_int] + _LOG_ARGS),
     "tl_sample_proc_log": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64,
-                                                    c_void_p, c_void_p, c_size_t] + _LOG_ARGS),
+                                                    c_void_p, c_void_p, c_size_t] + _LOG_ARGS + _WARP_ARGS),
     "tl_advance_pos": (c_int, [c_void_p, c_void_p, c_int, c_void_p]),
     "tl_append_token": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "tl_swiglu_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
@@ -508,20 +509,28 @@ def sample_ws(M: int) -> int:
     return int(load().tl_sample_ws(M))
 
 
+def _warp(min_p, typical_p, epsilon, eta):
+    """The sampler's trailing warper arguments (include/tensorlink_b200.h; off at 0, 1, 0, 0)."""
+    return float(min_p), float(typical_p), float(epsilon), float(eta)
+
+
 def sample(logits, ids_out, counters, ws, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
-           log=None):
-    """ids_out[m] ~ softmax(top-p(top-k(logits[m] / temperature))); ``counters`` int32[M] advance by one per call.
-    ``log``: None, or a score log (``_log_args``): raw logits, and logits / temperature on the kept set, -inf elsewhere."""
+           log=None, min_p: float = 0.0, typical_p: float = 1.0, epsilon: float = 0.0, eta: float = 0.0):
+    """ids_out[m] ~ softmax(eta(epsilon(typical(min-p(top-p(top-k(logits[m] / temperature))))))); ``counters`` int32[M]
+    advance by one per call.  ``log``: None, or a score log (``_log_args``): raw logits, and logits / temperature on the
+    kept set, -inf elsewhere.  ``min_p`` / ``typical_p`` / ``epsilon`` / ``eta``: HF's MinP / Typical / Epsilon / Eta
+    warpers, off at their defaults."""
     require_device()
     _bf16(logits)
     M, V = logits.shape
     assert ids_out.dtype == torch.int64 and counters.dtype == torch.int32 and counters.numel() >= M
     args = [_p(logits), _p(ids_out), M, V, float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1),
             _p(counters), _p(ws), ws.numel() * ws.element_size()]
+    warp = _warp(min_p, typical_p, epsilon, eta)
     if log is None:
-        _check(load().tl_sample(*args, _stream()), "tl_sample")
+        _check(load().tl_sample(*args, _stream(), *warp), "tl_sample")
     else:
-        _check(load().tl_sample_log(*args, *_log_args(log, M, V)), "tl_sample_log")
+        _check(load().tl_sample_log(*args, *_log_args(log, M, V), *warp), "tl_sample_log")
 
 
 def spec_accept_ws(K: int) -> int:
@@ -529,10 +538,11 @@ def spec_accept_ws(K: int) -> int:
 
 
 def spec_accept(p_logits, q_logits, in_ids, n_cand, counter, ids_out, ws, temperature: float = 1.0, top_k: int = 0,
-                top_p: float = 1.0, seed: int = 0):
+                top_p: float = 1.0, seed: int = 0, min_p: float = 0.0, typical_p: float = 1.0, epsilon: float = 0.0,
+                eta: float = 0.0):
     """Speculative sampling of one verify step: the target's rows p_logits [K+1, V_p], the assistant's q_logits [K, V_q]
-    (both bf16), the drafts in_ids[1..n_cand] drawn from q -> ids_out[0..n] in ``pl_accept``'s form (the kept drafts,
-    then the drawn token); ``counter`` int32[1] advances by one per call."""
+    (both bf16, each warped as ``sample`` warps it), the drafts in_ids[1..n_cand] drawn from q -> ids_out[0..n] in
+    ``pl_accept``'s form (the kept drafts, then the drawn token); ``counter`` int32[1] advances by one per call."""
     require_device()
     _bf16(p_logits, q_logits)
     K = q_logits.shape[0]
@@ -542,7 +552,8 @@ def spec_accept(p_logits, q_logits, in_ids, n_cand, counter, ids_out, ws, temper
     assert in_ids.dtype == torch.int64 and ids_out.dtype == torch.int64 and in_ids.numel() >= K + 1 and ids_out.numel() >= K + 1
     _check(load().tl_spec_accept(_p(p_logits), p_logits.shape[1], _p(q_logits), q_logits.shape[1], K, _p(in_ids), _p(n_cand),
                                  float(temperature), int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1), _p(counter),
-                                 _p(ids_out), _p(ws), ws.numel() * ws.element_size(), _stream()), "tl_spec_accept")
+                                 _p(ids_out), _p(ws), ws.numel() * ws.element_size(), _stream(),
+                                 *_warp(min_p, typical_p, epsilon, eta)), "tl_spec_accept")
 
 
 LP_PENALTY, LP_NGRAM, LP_MIN_NEW, LP_PROMPT, LP_N_EOS, LP_EOS, LP_MAX_EOS = 0, 1, 2, 3, 4, 5, 8
@@ -591,7 +602,8 @@ def argmax_proc(logits, ids_out, log, length, bits, params, ws, flags: int = 0, 
 
 
 def sample_proc(logits, ids_out, log, length, bits, params, counters, ws, temperature: float = 1.0, top_k: int = 0,
-                top_p: float = 1.0, seed: int = 0, flags: int = 0, score_log=None):
+                top_p: float = 1.0, seed: int = 0, flags: int = 0, score_log=None, min_p: float = 0.0, typical_p: float = 1.0,
+                epsilon: float = 0.0, eta: float = 0.0):
     """``sample`` over HF's processed fp32 scores; appends the drawn id to row m's history.  ``score_log``: None, or a
     score log (``_log_args``): raw logits, and processed / temperature on the kept set, -inf elsewhere."""
     require_device()
@@ -602,10 +614,11 @@ def sample_proc(logits, ids_out, log, length, bits, params, counters, ws, temper
     assert params.dtype == torch.int32 and params.numel() >= LP_PARAMS
     args = [_p(logits), _p(ids_out), _p(log), _p(length), _p(bits), _p(params), flags, M, V, L, float(temperature),
             int(top_k or 0), float(top_p), int(seed) & (2 ** 64 - 1), _p(counters), _p(ws), ws.numel() * ws.element_size()]
+    warp = _warp(min_p, typical_p, epsilon, eta)
     if score_log is None:
-        _check(load().tl_sample_proc(*args, _stream()), "tl_sample_proc")
+        _check(load().tl_sample_proc(*args, _stream(), *warp), "tl_sample_proc")
     else:
-        _check(load().tl_sample_proc_log(*args, *_log_args(score_log, M, V)), "tl_sample_proc_log")
+        _check(load().tl_sample_proc_log(*args, *_log_args(score_log, M, V), *warp), "tl_sample_proc_log")
 
 
 def lp_params(penalty: float, ngram: int, min_new: int, prompt_len: int, eos_ids) -> torch.Tensor:
