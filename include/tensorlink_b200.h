@@ -439,6 +439,32 @@ int tl_adamw_step(void* param, const void* grad, float* exp_avg, float* exp_avg_
                   float beta1, float beta2, float eps, float weight_decay, int step, int decoupled,
                   void* stream);
 
+
+/* ---- Qwen3-MoE sparse MLP (HF Qwen3MoeSparseMoeBlock with eager experts; tensorlink_b200/csrc/moe.cu)
+ * tl_moe_route: per token (N rows of bf16 logits [N,E], E <= 256, 1 <= k <= min(16,E)): the top-k of the fp32 softmax,
+ *   ties toward the lower expert, ids[N,k] sorted ascending and wts[N,k] fp32 (renormalised over the picks if
+ *   norm_topk).  counts/offsets/row_of/tiles (all or none): the grouped-GEMM plan — counts[E], offsets[E+1] (segments
+ *   padded to 128 rows), row_of[N*k] (token, slot) -> segment row in ascending token order, tiles[max_tiles][2] =
+ *   (expert or -1, valid rows) per 128-row M-tile; max_tiles >= tl_moe_max_tiles(N, E, k).
+ * tl_moe_gather: hg[row_of[t*k+s], :] = h[t, :].
+ * tl_moe_gemm: C[r, :] = A[r, :] · W[e]^T (W [E*N, K], expert e = rows e*N..) for the valid rows of every tile; flags
+ *   0 (bf16 out) or TL_EPI_SWIGLU (interleaved gate/up rows, C [rows, N/2]); N % 128 == 0.
+ * tl_moe_combine: out[t] = bf16(x[t] + acc), acc = +0 then acc = bf16(acc + bf16(y[row_of[t*k+s]] * wts[t,s])) for
+ *   s = 0..k-1 (ascending expert).  out may alias x.
+ * tl_moe_gemv: M <= 16 decode rows, weights of the picked experts only.  TL_EPI_SWIGLU: y[M*k, N/2] per (row, pick)
+ *   from x[M,K] and W [E, N, K] with interleaved gate/up rows.  TL_EPI_RESIDUAL: x = act [M*k, K], W [E, N, K];
+ *   y[M, N] = the combine above with residual [M, N] (y may alias residual). */
+int tl_moe_max_tiles(int N, int E, int k);
+int tl_moe_route(const void* logits, int N, int E, int k, int norm_topk, int32_t* ids, float* wts, int32_t* counts,
+                 int32_t* offsets, int32_t* row_of, int32_t* tiles, int max_tiles, void* stream);
+int tl_moe_gather(const void* h, const int32_t* row_of, void* hg, int N, int k, int H, void* stream);
+int tl_moe_gemm(const void* A, const void* W, void* C, const int32_t* tiles, int max_tiles, int E, int N, int K, int ldc,
+                int flags, void* stream);
+int tl_moe_combine(const void* y, const int32_t* row_of, const float* wts, const void* x, void* out, int N, int k, int H,
+                   void* stream);
+int tl_moe_gemv(const void* x, const void* W, void* y, const int32_t* ids, const float* wts, const void* residual, int M,
+                int k, int N, int K, int flags, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

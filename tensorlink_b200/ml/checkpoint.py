@@ -18,7 +18,7 @@ from typing import Dict, Iterator
 import torch
 
 from . import fp8 as F8
-from .configs import ShardModelConfig
+from .configs import ShardModelConfig, check_moe, moe_fields
 
 INDEX = "model.safetensors.index.json"
 SINGLE = "model.safetensors"
@@ -38,17 +38,22 @@ def config_from_dir(path: str) -> ShardModelConfig:
         c = json.load(f)
     quantization_from_dir(path)
     mt = c.get("model_type", "")
-    if mt not in ("qwen2", "qwen3"):
-        raise ValueError(f"{path}: model_type {mt!r} is not supported (qwen2 / qwen3)")
-    qk_norm = mt == "qwen3"
+    moe = moe_fields(mt, c.get)
+    if mt not in ("qwen2", "qwen3", "qwen3_moe"):
+        raise ValueError(f"{path}: model_type {mt!r} is not supported (qwen2 / qwen3 / qwen3_moe)")
+    if moe and c.get("quantization_config"):
+        raise NotImplementedError(f"{path}: FP8 Qwen3-MoE checkpoints are not supported")
+    qk_norm = mt in ("qwen3", "qwen3_moe")
     n_h = int(c["num_attention_heads"])
     hd = int(c.get("head_dim") or c["hidden_size"] // n_h)
     theta = (c.get("rope_parameters") or {}).get("rope_theta", c.get("rope_theta", 1e6))
-    return ShardModelConfig(c.get("_name_or_path") or os.path.basename(os.path.normpath(path)), int(c["hidden_size"]),
-                            int(c["intermediate_size"]), int(c["num_hidden_layers"]), n_h, int(c["num_key_value_heads"]), hd,
-                            int(c["vocab_size"]), tied=bool(c.get("tie_word_embeddings", False)), qkv_bias=not qk_norm,
-                            qk_norm=qk_norm, rope_theta=float(theta), rms_eps=float(c.get("rms_norm_eps", 1e-6)),
-                            max_pos=int(c.get("max_position_embeddings", 32768)))
+    cfg = ShardModelConfig(c.get("_name_or_path") or os.path.basename(os.path.normpath(path)), int(c["hidden_size"]),
+                           int(c["intermediate_size"]), int(c["num_hidden_layers"]), n_h, int(c["num_key_value_heads"]), hd,
+                           int(c["vocab_size"]), tied=bool(c.get("tie_word_embeddings", False)), qkv_bias=not qk_norm,
+                           qk_norm=qk_norm, rope_theta=float(theta), rms_eps=float(c.get("rms_norm_eps", 1e-6)),
+                           max_pos=int(c.get("max_position_embeddings", 32768)), **moe)
+    check_moe(cfg)
+    return cfg
 
 
 def config_to_json(cfg: ShardModelConfig) -> dict:
@@ -58,7 +63,32 @@ def config_to_json(cfg: ShardModelConfig) -> dict:
             "num_key_value_heads": cfg.n_kv_heads, "head_dim": cfg.head_dim, "vocab_size": cfg.vocab,
             "tie_word_embeddings": bool(cfg.tied), "rope_theta": cfg.rope_theta, "rms_norm_eps": cfg.rms_eps,
             "max_position_embeddings": cfg.max_pos, "hidden_act": "silu", "torch_dtype": "bfloat16",
-            "attention_bias": bool(cfg.qkv_bias), "_name_or_path": cfg.name}
+            "attention_bias": bool(cfg.qkv_bias), "_name_or_path": cfg.name,
+            **({"architectures": ["Qwen3MoeForCausalLM"], "model_type": "qwen3_moe", "num_experts": cfg.n_experts,
+                "num_experts_per_tok": cfg.top_k, "moe_intermediate_size": cfg.moe_intermediate,
+                "norm_topk_prob": bool(cfg.norm_topk_prob), "decoder_sparse_step": 1, "mlp_only_layers": []}
+               if cfg.is_moe else {})}
+
+
+def _per_expert(cfg: ShardModelConfig, sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """HF's fused in-memory expert tensors -> the per-expert names Qwen3-MoE checkpoints store."""
+    if not cfg.is_moe:
+        return sd
+    out: Dict[str, torch.Tensor] = {}
+    Ie = cfg.moe_intermediate
+    for k, t in sd.items():
+        if k.endswith("mlp.experts.gate_up_proj"):
+            pre = k[:-len("gate_up_proj")]
+            for e in range(cfg.n_experts):
+                out[f"{pre}{e}.gate_proj.weight"] = t[e, :Ie].contiguous()
+                out[f"{pre}{e}.up_proj.weight"] = t[e, Ie:].contiguous()
+        elif k.endswith("mlp.experts.down_proj"):
+            pre = k[:-len("down_proj")]
+            for e in range(cfg.n_experts):
+                out[f"{pre}{e}.down_proj.weight"] = t[e].contiguous()
+        else:
+            out[k] = t
+    return out
 
 
 class LazyCheckpoint:
@@ -107,7 +137,7 @@ def save_checkpoint(dm, path: str, link=None) -> None:
     from safetensors.torch import save_file
     link = link or dm.link
     os.makedirs(path, exist_ok=True)
-    sd = {k: v.detach().to("cpu").contiguous() for k, v in dm.stage.params.hf_state_dict().items()}
+    sd = _per_expert(dm.cfg, {k: v.detach().to("cpu").contiguous() for k, v in dm.stage.params.hf_state_dict().items()})
     if dm.cfg.tied and "lm_head.weight" in sd and "model.embed_tokens.weight" in sd:
         sd.pop("lm_head.weight")                    # tied: stored once, like HF
     fn = f"model-{link.rank + 1:05d}-of-{link.world:05d}.safetensors"

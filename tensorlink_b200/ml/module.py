@@ -26,7 +26,7 @@ from ..native import LP_MAX_EOS, PL_MAX_DRAFT, PL_MAX_EOS
 from ..p2p.link import StageLink, init_process_group_from_env
 from . import fp8 as F8
 from . import graphing
-from .configs import ShardModelConfig, get_config
+from .configs import ShardModelConfig, check_moe, get_config, moe_fields
 
 
 @dataclass
@@ -47,6 +47,7 @@ def _default_stage_factory(**kw):
 def _config_from_hf(model) -> ShardModelConfig:
     c = model.config
     qk_norm = c.__class__.__name__.startswith("Qwen3")
+    moe = moe_fields(getattr(c, "model_type", ""), lambda k: getattr(c, k, None))
     hd = getattr(c, "head_dim", None) or c.hidden_size // c.num_attention_heads
     rp = getattr(c, "rope_parameters", None) or {}
     theta = rp.get("rope_theta", getattr(c, "rope_theta", 1e6))
@@ -54,7 +55,7 @@ def _config_from_hf(model) -> ShardModelConfig:
                             c.intermediate_size, c.num_hidden_layers, c.num_attention_heads,
                             c.num_key_value_heads, hd, c.vocab_size, tied=bool(c.tie_word_embeddings),
                             qkv_bias=not qk_norm, qk_norm=qk_norm, rope_theta=float(theta),
-                            rms_eps=float(c.rms_norm_eps), max_pos=int(c.max_position_embeddings))
+                            rms_eps=float(c.rms_norm_eps), max_pos=int(c.max_position_embeddings), **moe)
 
 
 # HF forward / generate keywords that change nothing here when left at these values (anything else raises instead of
@@ -396,6 +397,12 @@ class DistributedModel(torch.nn.Module):
             self.cfg = get_config(model)
         if quantization is not None and training:
             raise NotImplementedError("training with FP8 weights is not supported: load an FP8 model with training=False")
+        if self.cfg.is_moe:
+            check_moe(self.cfg)
+            if training:
+                raise NotImplementedError("training a Qwen3-MoE model is not supported: load it with training=False")
+            if quantization is not None:
+                raise NotImplementedError("FP8 Qwen3-MoE weights are not supported: load the bf16 checkpoint")
         self.quantization = quantization
         self.model_name = self.cfg.name
         self.name = self.model_name
@@ -495,6 +502,8 @@ class DistributedModel(torch.nn.Module):
         save_checkpoint(self, path)
 
     def create_optimizer(self, **optimizer_kwargs):
+        if self.cfg.is_moe:
+            raise NotImplementedError("training a Qwen3-MoE model is not supported (no optimizer for a MoE model)")
         if self.quantization is not None:
             raise NotImplementedError("training with FP8 weights is not supported (no optimizer for an FP8 model)")
         from .optim import create_distributed_optimizer

@@ -26,7 +26,7 @@ import torch
 
 from .. import native as nat
 from . import fp8 as F8
-from .configs import ShardModelConfig
+from .configs import ShardModelConfig, check_moe
 from .weights import init_state_dict
 
 ALIGN = 128  # elements (256 B)
@@ -88,6 +88,10 @@ class ShardParams:
                  device, with_grad: bool = False, fp8: bool = False):
         if fp8 and with_grad:
             raise NotImplementedError("training with FP8 weights is not supported (load the model with training=False)")
+        check_moe(cfg)
+        if cfg.is_moe and (fp8 or with_grad):
+            raise NotImplementedError("a Qwen3-MoE model runs bf16 inference only: " +
+                                      ("FP8 MoE weights are not supported" if fp8 else "training is not supported"))
         self.fp8 = bool(fp8)
         self.cfg, self.layer_ids = cfg, list(layer_ids)
         self.has_embed, self.has_head = has_embed, has_head
@@ -100,8 +104,12 @@ class ShardParams:
                 spec.append((f"l{li}.bqkv", (cfg.qkv_dim,)))
             if cfg.qk_norm:
                 spec += [(f"l{li}.qn", (cfg.head_dim,)), (f"l{li}.kn", (cfg.head_dim,))]
-            spec += [(f"l{li}.wo", (H, cfg.q_dim)), (f"l{li}.ln2", (H,)), (f"l{li}.wgu", (2 * I, H)),
-                     (f"l{li}.wd", (H, I))]
+            spec += [(f"l{li}.wo", (H, cfg.q_dim)), (f"l{li}.ln2", (H,))]
+            if cfg.is_moe:
+                E, Ie = cfg.n_experts, cfg.moe_intermediate
+                spec += [(f"l{li}.router", (E, H)), (f"l{li}.ewgu", (E, 2 * Ie, H)), (f"l{li}.ewd", (E, H, Ie))]
+            else:
+                spec += [(f"l{li}.wgu", (2 * I, H)), (f"l{li}.wd", (H, I))]
         if has_embed:
             spec.append(("embed", (cfg.vocab, H)))
         if has_head:
@@ -169,7 +177,10 @@ class ShardParams:
                 put(f"l{li}.qn", sd[p + "self_attn.q_norm.weight"])
                 put(f"l{li}.kn", sd[p + "self_attn.k_norm.weight"])
             put(f"l{li}.ln2", sd[p + "post_attention_layernorm.weight"])
-            if not self.fp8:
+            if cfg.is_moe:
+                put(f"l{li}.wo", sd[p + "self_attn.o_proj.weight"])
+                self._load_experts(sd, li)
+            elif not self.fp8:
                 put(f"l{li}.wo", sd[p + "self_attn.o_proj.weight"])
                 g, u = sd[p + "mlp.gate_proj.weight"], sd[p + "mlp.up_proj.weight"]
                 put(f"l{li}.wgu", torch.stack([g, u], dim=1).reshape(2 * cfg.intermediate, cfg.hidden))
@@ -204,6 +215,13 @@ class ShardParams:
                 out[p + "self_attn.k_norm.weight"] = src[f"l{li}.kn"].clone()
             out[p + "self_attn.o_proj.weight"] = src[f"l{li}.wo"].clone()
             out[p + "post_attention_layernorm.weight"] = src[f"l{li}.ln2"].clone()
+            if cfg.is_moe:
+                E, Ie, H = cfg.n_experts, cfg.moe_intermediate, cfg.hidden
+                gu = src[f"l{li}.ewgu"].view(E, Ie, 2, H)
+                out[p + "mlp.gate.weight"] = src[f"l{li}.router"].clone()
+                out[p + "mlp.experts.gate_up_proj"] = torch.cat([gu[:, :, 0], gu[:, :, 1]], dim=1)
+                out[p + "mlp.experts.down_proj"] = src[f"l{li}.ewd"].clone()
+                continue
             gu = src[f"l{li}.wgu"].view(cfg.intermediate, 2, cfg.hidden)
             out[p + "mlp.gate_proj.weight"], out[p + "mlp.up_proj.weight"] = gu[:, 0].clone(), gu[:, 1].clone()
             out[p + "mlp.down_proj.weight"] = src[f"l{li}.wd"].clone()
@@ -214,6 +232,27 @@ class ShardParams:
             # tied heads appear under both names, like HF's own state_dict()
             out["lm_head.weight"] = out["model.embed_tokens.weight"] if (cfg.tied and self.has_embed) else src["head"].clone()
         return self._with_scale_grids(out) if self.fp8 else out
+
+    def _load_experts(self, sd, li: int):
+        """Layer li's router and experts, from HF's fused in-memory names (``mlp.experts.gate_up_proj`` [E, 2I, H] with
+        the gate rows first, ``mlp.experts.down_proj`` [E, H, I]) or the checkpoints' per-expert names
+        (``mlp.experts.{e}.{gate,up,down}_proj.weight``).  Gate/up rows are interleaved per expert as in ``wgu``."""
+        cfg, p = self.cfg, f"model.layers.{li}."
+        E, Ie, H = cfg.n_experts, cfg.moe_intermediate, cfg.hidden
+        dev = self.device
+        self.v[f"l{li}.router"].copy_(sd[p + "mlp.gate.weight"].to(device=dev, dtype=torch.bfloat16))
+        gu, dn = self.v[f"l{li}.ewgu"].view(E, Ie, 2, H), self.v[f"l{li}.ewd"]
+        if p + "mlp.experts.gate_up_proj" in sd:
+            w = sd[p + "mlp.experts.gate_up_proj"].to(device=dev, dtype=torch.bfloat16)
+            gu[:, :, 0].copy_(w[:, :Ie])
+            gu[:, :, 1].copy_(w[:, Ie:])
+            dn.copy_(sd[p + "mlp.experts.down_proj"].to(device=dev, dtype=torch.bfloat16))
+            return
+        for e in range(E):
+            q = f"{p}mlp.experts.{e}."
+            gu[e, :, 0].copy_(sd[q + "gate_proj.weight"].to(device=dev, dtype=torch.bfloat16))
+            gu[e, :, 1].copy_(sd[q + "up_proj.weight"].to(device=dev, dtype=torch.bfloat16))
+            dn[e].copy_(sd[q + "down_proj.weight"].to(device=dev, dtype=torch.bfloat16))
 
     def _load_linears_fp8(self, sd, li: int):
         """Layer li's four Linears from HF's FP8 weight + scale_inv grid of each projection (a bf16 weight is quantized
@@ -302,6 +341,25 @@ class ShardBuffers:
     q: torch.Tensor
     attn: torch.Tensor
     act: torch.Tensor
+    moe: Optional["MoeBuffers"] = None        # routing buffers of a MoE stage
+
+
+class MoeBuffers:
+    """Routing buffers of a Qwen3-MoE stage for up to ``n`` tokens: router logits, the picks and their weights, the
+    grouped-GEMM plan (csrc/moe.cu) and the gathered rows; decode rows use ``act[:n*k]`` for their expert activations."""
+
+    def __init__(self, cfg: ShardModelConfig, n: int, device):
+        E, k, H, Ie = cfg.n_experts, cfg.top_k, cfg.hidden, cfg.moe_intermediate
+        i32 = dict(dtype=torch.int32, device=device)
+        self.n, self.tiles_max = n, nat.moe_max_tiles(n, E, k)
+        rows = self.tiles_max * 128
+        self.logits = torch.empty(n, E, dtype=torch.bfloat16, device=device)
+        self.ids, self.wts = torch.empty(n, k, **i32), torch.empty(n, k, dtype=torch.float32, device=device)
+        self.counts, self.offsets, self.row_of = torch.empty(E, **i32), torch.empty(E + 1, **i32), torch.empty(n * k, **i32)
+        self.tiles = torch.empty(self.tiles_max, 2, **i32)
+        self.hg = torch.empty(rows, H, dtype=torch.bfloat16, device=device)
+        self.act = torch.empty(rows, Ie, dtype=torch.bfloat16, device=device)
+        self.y = torch.empty(rows, H, dtype=torch.bfloat16, device=device)
 
 
 class CudaLayerGroup:
@@ -334,6 +392,9 @@ class CudaLayerGroup:
         self.n_max = max_tokens or max_batch * max_seq
         self._alloc_bufs(min(self.n_max, 8))
         self.dbufs = self._make_bufs(max_batch)       # decode-time buffers: fixed addresses (captured graphs, job lists)
+        self.moe_pf: Optional[MoeBuffers] = None
+        if cfg.is_moe:
+            self.dbufs.moe = MoeBuffers(cfg, max_batch, dev)
         # ticket counters of the four decode GEMVs of every layer (_layer_decode): one block per call site, so no two
         # launches that can overlap share one, and captured graphs keep fixed addresses
         self.gemv_ctr = nat.gemv_counters(self.num_layers, 4, device=dev)
@@ -365,13 +426,15 @@ class CudaLayerGroup:
 
     def _dbufs(self, n: int) -> ShardBuffers:
         b = self.dbufs
-        return ShardBuffers(b.x[:n], b.h[:n], b.qkv[:n], b.q[:n], b.attn[:n], b.act[:n])
+        return ShardBuffers(b.x[:n], b.h[:n], b.qkv[:n], b.q[:n], b.attn[:n], b.act[:n], b.moe)
 
     def _bufs(self, n: int) -> ShardBuffers:
         if n > self.n_alloc:
             self._alloc_bufs(n)
         b = self.bufs
-        return ShardBuffers(b.x[:n], b.h[:n], b.qkv[:n], b.q[:n], b.attn[:n], b.act[:n])
+        if self.cfg.is_moe and (self.moe_pf is None or self.moe_pf.n < n):
+            self.moe_pf = MoeBuffers(self.cfg, n, self.device)
+        return ShardBuffers(b.x[:n], b.h[:n], b.qkv[:n], b.q[:n], b.attn[:n], b.act[:n], self.moe_pf)
 
     # ------------------------------------------------------------------------------------------ cache control
     def reset_cache(self, past_len: int = 0):
@@ -413,8 +476,42 @@ class CudaLayerGroup:
                              cfg.head_dim, self.scale, kv_start=ks)
         self._gemm(w.attn, f"l{li}.wo", out=x, residual=x)
         nat.rmsnorm_fwd(x, v[f"l{li}.ln2"], cfg.rms_eps, out=w.h)
+        if cfg.is_moe:
+            self._moe_grouped(li, x, w.h, w.moe)
+            return
         self._gemm(w.h, f"l{li}.wgu", out=w.act, flags=nat.EPI_SWIGLU)
         self._gemm(w.act, f"l{li}.wd", out=x, residual=x)
+
+    def _moe_grouped(self, li: int, x: torch.Tensor, h: torch.Tensor, mb: MoeBuffers, out: Optional[torch.Tensor] = None):
+        """Qwen3-MoE block for the N rows of ``h`` (the normed ``x``): router GEMM -> route + plan -> gather -> grouped
+        gate/up (SwiGLU) -> grouped down -> combine, out = bf16(x + acc) (into ``x`` unless ``out``)."""
+        cfg, v = self.cfg, self.p.v
+        n, k = h.shape[0], cfg.top_k
+        T = nat.moe_max_tiles(n, cfg.n_experts, k)
+        nat.gemm(h, v[f"l{li}.router"], out=mb.logits[:n])
+        row_of, tiles = mb.row_of[:n * k], mb.tiles[:T]
+        nat.moe_route(mb.logits[:n], k, cfg.norm_topk_prob, mb.ids[:n], mb.wts[:n], (mb.counts, mb.offsets, row_of, tiles))
+        nat.moe_gather(h, row_of, mb.hg[:T * 128], k)
+        nat.moe_gemm(mb.hg[:T * 128], v[f"l{li}.ewgu"], mb.act[:T * 128], tiles, flags=nat.EPI_SWIGLU)
+        nat.moe_gemm(mb.act[:T * 128], v[f"l{li}.ewd"], mb.y[:T * 128], tiles)
+        nat.moe_combine(mb.y[:T * 128], row_of, mb.wts[:n], x, x if out is None else out)
+
+    def _layer_decode_moe(self, j: int, x: torch.Tensor, B: int, w: ShardBuffers, out: Optional[torch.Tensor], attention):
+        """``_layer_decode`` of a MoE layer: the attention half as in the dense layer, then norm -> router GEMV -> route ->
+        expert GEMV gate/up over the picked experts only -> expert GEMV down with the combine and the residual."""
+        cfg, v, li, mb = self.cfg, self.p.v, self.layer_ids[j], w.moe
+        ctr = self.gemv_ctr[j]
+        self._gemv(x, f"l{li}.wqkv", out=w.qkv, bias=v.get(f"l{li}.bqkv"), norm_w=v[f"l{li}.ln1"], eps=cfg.rms_eps,
+                   next_w=v[f"l{li}.wo"], counter=ctr[0])
+        attention(j, li, B, w)
+        self._gemv(w.attn, f"l{li}.wo", out=x, residual=x, next_w=v[f"l{li}.router"], counter=ctr[1])
+        nat.rmsnorm_fwd(x, v[f"l{li}.ln2"], cfg.rms_eps, out=w.h)
+        nat.gemv(w.h, v[f"l{li}.router"], out=mb.logits[:B], counter=ctr[2])
+        nat.moe_route(mb.logits[:B], cfg.top_k, cfg.norm_topk_prob, mb.ids[:B], mb.wts[:B])
+        act = mb.act[:B * cfg.top_k]
+        nat.moe_gemv(w.h, v[f"l{li}.ewgu"], act, mb.ids[:B], flags=nat.EPI_SWIGLU)
+        nat.moe_gemv(act, v[f"l{li}.ewd"], x if out is None else out, mb.ids[:B], wts=mb.wts[:B], residual=x,
+                     flags=nat.EPI_RESIDUAL)
 
     FUSED_DECODE_MAX_T = 2048
 
@@ -439,6 +536,8 @@ class CudaLayerGroup:
         ``attention``: what turns w.qkv into w.attn instead of ``_decode_attention`` (the verify step's)."""
         cfg, v, li = self.cfg, self.p.v, self.layer_ids[j]
         attention = attention or self._decode_attention
+        if cfg.is_moe:
+            return self._layer_decode_moe(j, x, B, w, out, attention)
         # every GEMV names the weights of the launch after it: it queues L2 prefetches behind its own loads, so HBM keeps
         # streaming through the launch boundary (and through the attention kernel) instead of idling there
         if j + 1 < self.num_layers:
@@ -463,6 +562,13 @@ class CudaLayerGroup:
         cfg, v, li = self.cfg, self.p.v, self.layer_ids[j]
         if ws is None:
             ws = self.gemm_ws if B <= 128 else None
+        if cfg.is_moe:
+            nat.rmsnorm_fwd(x, v[f"l{li}.ln1"], cfg.rms_eps, out=w.h)
+            self._gemm(w.h, f"l{li}.wqkv", out=w.qkv, bias=v.get(f"l{li}.bqkv"), ws=ws)
+            (attention or self._decode_attention)(j, li, B, w)
+            self._gemm(w.attn, f"l{li}.wo", out=x, residual=x, ws=ws, norm_w=v[f"l{li}.ln2"], eps=cfg.rms_eps, h_out=w.h)
+            self._moe_grouped(li, x, w.h, w.moe, out if j == self.num_layers - 1 else None)
+            return
         if j == 0:
             nat.rmsnorm_fwd(x, v[f"l{li}.ln1"], cfg.rms_eps, out=w.h)
         self._gemm(w.h, f"l{li}.wqkv", out=w.qkv, bias=v.get(f"l{li}.bqkv"), ws=ws)
@@ -556,11 +662,13 @@ class CudaLayerGroup:
         if self.vbufs is None:
             cfg, dev, R = self.cfg, self.device, nat.VERIFY_MAX_ROWS
             self.vbufs = self._make_bufs(R)
+            if cfg.is_moe:
+                self.vbufs.moe = MoeBuffers(cfg, R, dev)
             self.ver_gemm_ws = torch.empty(nat.gemm_splitk_ws(R, max(cfg.qkv_dim, cfg.hidden)), dtype=torch.uint8, device=dev)
             self.ver_attn_ws = torch.empty(nat.attn_verify_ws(R, cfg.n_heads, cfg.head_dim, self.T_max), dtype=torch.uint8,
                                            device=dev)
         b = self.vbufs
-        w = ShardBuffers(b.x[:n], b.h[:n], b.qkv[:n], b.q[:n], b.attn[:n], b.act[:n])
+        w = ShardBuffers(b.x[:n], b.h[:n], b.qkv[:n], b.q[:n], b.attn[:n], b.act[:n], b.moe)
         for j in range(self.num_layers):
             if n <= self.gemv_rows():
                 self._layer_decode(j, x, n, w, attention=self._verify_attention)
@@ -577,7 +685,7 @@ class CudaLayerGroup:
         # the chain's ATTN job has no per-row key start: a left-padded slot takes the per-kernel sequence
         # the chain's GEMV jobs stream bf16 weights: an FP8 shard takes the per-kernel sequence
         return (os.environ.get("TL_DECODE_IMPL", "kernels") == "chain" and self.allow_chain and self.num_layers > 0
-                and not self.ragged and not self.p.fp8
+                and not self.ragged and not self.p.fp8 and not cfg.is_moe
                 and B <= min(4, gemv_max_rows()) and cfg.n_kv_heads * B <= 60 and cfg.n_heads // cfg.n_kv_heads <= 8
                 and cfg.head_dim in (64, 128) and self._chain_ring_fits(B))
 
@@ -650,7 +758,7 @@ class CudaLayerGroup:
         long and a short weight stream)."""
         import os
         return (os.environ.get("TL_DECODE_IMPL", "kernels") == "dq" and self.allow_chain and self.num_layers > 1
-                and B <= min(4, gemv_max_rows()) and not self.p.fp8 and self._chain_ring_fits(B))
+                and B <= min(4, gemv_max_rows()) and not self.p.fp8 and not self.cfg.is_moe and self._chain_ring_fits(B))
 
     def _decode_step_dq(self, x: torch.Tensor, B: int, out: Optional[torch.Tensor]):
         cfg, v = self.cfg, self.p.v

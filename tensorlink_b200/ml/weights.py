@@ -41,10 +41,14 @@ def layer_param_shapes(cfg: ShardModelConfig) -> Dict[str, tuple]:
         "self_attn.v_proj.weight": (cfg.kv_dim, H),
         "self_attn.o_proj.weight": (H, cfg.q_dim),
         "post_attention_layernorm.weight": (H,),
-        "mlp.gate_proj.weight": (I, H),
-        "mlp.up_proj.weight": (I, H),
-        "mlp.down_proj.weight": (H, I),
     }
+    if cfg.is_moe:
+        # HF's in-memory (fused) expert layout; the checkpoints on disk hold one tensor per expert (ml/shard.py)
+        E, Ie = cfg.n_experts, cfg.moe_intermediate
+        s.update({"mlp.gate.weight": (E, H), "mlp.experts.gate_up_proj": (E, 2 * Ie, H),
+                  "mlp.experts.down_proj": (E, H, Ie)})
+    else:
+        s.update({"mlp.gate_proj.weight": (I, H), "mlp.up_proj.weight": (I, H), "mlp.down_proj.weight": (H, I)})
     if cfg.qkv_bias:
         s["self_attn.q_proj.bias"] = (cfg.q_dim,)
         s["self_attn.k_proj.bias"] = (cfg.kv_dim,)

@@ -126,6 +126,14 @@ _SIGS = {
     "tl_add_inplace": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "tl_scale_add_bf16": (c_int, [c_void_p, c_void_p, c_float, c_int, c_size_t, c_void_p]),
     "tl_scale_add_f32": (c_int, [c_void_p, c_void_p, c_float, c_int, c_size_t, c_void_p]),
+    "tl_moe_max_tiles": (c_int, [c_int, c_int, c_int]),
+    "tl_moe_route": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                             c_void_p, c_int, c_void_p]),
+    "tl_moe_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "tl_moe_gemm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "tl_moe_combine": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "tl_moe_gemv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                            c_void_p]),
     "tl_adamw_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_float, c_float, c_float, c_float,
                               c_float, c_int, c_int, c_void_p]),
 }
@@ -914,3 +922,58 @@ def qk_norm_bwd(qkv_pre, dqkv, qn, kn, dqn_acc, dkn_acc, eps, n_h, n_kv, d):
     require_device(); _bf16(qkv_pre, dqkv, qn, kn)
     _check(load().tl_qk_norm_bwd(_p(qkv_pre), _p(dqkv), _p(qn), _p(kn), _p(dqn_acc), _p(dkn_acc), eps, dqkv.shape[0], n_h,
                                  n_kv, d, _stream()), "tl_qk_norm_bwd")
+
+
+# ---------------------------------------------------------------------------------------------- Qwen3-MoE (csrc/moe.cu)
+def moe_max_tiles(N: int, E: int, k: int) -> int:
+    """128-row M-tiles the grouped GEMM of N tokens may need (every non-empty expert segment padded to a tile)."""
+    return int(load().tl_moe_max_tiles(N, E, k))
+
+
+def moe_route(logits: torch.Tensor, k: int, norm_topk: bool, ids: torch.Tensor, wts: torch.Tensor, plan=None):
+    """Top-k routing of ``logits`` [N,E] bf16 into ``ids`` [N,k] int32 (ascending) and ``wts`` [N,k] fp32.  ``plan``:
+    (counts [E], offsets [E+1], row_of [N*k], tiles [T,2]) int32 tensors for the grouped GEMM, or None."""
+    require_device()
+    _bf16(logits)
+    N, E = logits.shape
+    assert ids.dtype == torch.int32 and wts.dtype == torch.float32
+    counts, offsets, row_of, tiles = plan if plan is not None else (None, None, None, None)
+    _check(load().tl_moe_route(_p(logits), N, E, k, int(bool(norm_topk)), _p(ids), _p(wts), _p(counts), _p(offsets),
+                               _p(row_of), _p(tiles), 0 if tiles is None else tiles.shape[0], _stream()), "tl_moe_route")
+
+
+def moe_gather(h: torch.Tensor, row_of: torch.Tensor, hg: torch.Tensor, k: int):
+    require_device()
+    _bf16(h, hg)
+    _check(load().tl_moe_gather(_p(h), _p(row_of), _p(hg), h.shape[0], k, h.shape[1], _stream()), "tl_moe_gather")
+    return hg
+
+
+def moe_gemm(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, tiles: torch.Tensor, flags: int = 0):
+    """Grouped GEMM: ``w`` [E, N, K]; M-tile t of ``a`` [tiles*128, K] runs on expert tiles[t, 0]."""
+    require_device()
+    _bf16(a, w, out)
+    E, N, K = w.shape
+    _check(load().tl_moe_gemm(_p(a), _p(w), _p(out), _p(tiles), tiles.shape[0], E, N, K, out.stride(0), flags, _stream()),
+           "tl_moe_gemm")
+    return out
+
+
+def moe_combine(y: torch.Tensor, row_of: torch.Tensor, wts: torch.Tensor, x: torch.Tensor, out: torch.Tensor):
+    require_device()
+    _bf16(y, x, out)
+    N, k = wts.shape
+    _check(load().tl_moe_combine(_p(y), _p(row_of), _p(wts), _p(x), _p(out), N, k, x.shape[1], _stream()), "tl_moe_combine")
+    return out
+
+
+def moe_gemv(x: torch.Tensor, w: torch.Tensor, out: torch.Tensor, ids: torch.Tensor, *, wts=None, residual=None,
+             flags: int = EPI_SWIGLU):
+    """Expert GEMV over the picked experts ``ids`` [M,k] of ``w`` [E, N, K] (see tl_moe_gemv)."""
+    require_device()
+    _bf16(x, w, out, residual)
+    E, N, K = w.shape
+    M, k = ids.shape
+    _check(load().tl_moe_gemv(_p(x), _p(w), _p(out), _p(ids), _p(wts), _p(residual), M, k, N, K, flags, _stream()),
+           "tl_moe_gemv")
+    return out
